@@ -10,7 +10,8 @@ configs[2]).  The JSON line carries
                to 16-byte pixels (one rank) or raw row slices + NVLink all-gather (more ranks), H2D and a D2H read of
                the per-step result inside the timed region,
   host_load_leg the device-resident leg again with every host core busy (median of three repeats),
-  roofline     achieved algorithmic GB/s of the dominant kernel against the measured HBM peak,
+  roofline     achieved algorithmic GB/s of the dominant kernel against the HBM peak (MEASURED_PEAKS.json when present,
+               else the H100 SXM data sheet's 3.35 TB/s; `peak_source` says which),
   cpu_baseline the reference's CPU path timed on this box's host cores (bounded sample).
 `--impl reference` times the CPU arm alone (oracle/_ref = the reference's own sources when they
 compiled here, else the oracle port).  Under torchrun (N > 1) the volume is sharded by coarse
@@ -34,7 +35,7 @@ sys.path.insert(0, ROOT)
 from cpu_tsdf_b200 import synth  # noqa: E402
 
 FRAMES_PER_STEP = 32
-N_DISTINCT = 64            # distinct frames/poses cycled through (inputs 64 x 9.8 MB = 629 MB > 126 MB L2)
+N_DISTINCT = 64            # distinct frames/poses cycled through (inputs 64 x 9.8 MB = 629 MB > 50 MB L2)
 RES, SIZE = 2048, 10.0
 CAM = synth.Camera()
 SCENE = synth.S2
@@ -75,7 +76,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
@@ -236,12 +237,38 @@ def run_reference(args, rank, world):
     print(json.dumps(line))
 
 
+DUMP_SAMPLE = 32           # keep the nodes whose key hash is 0 mod DUMP_SAMPLE ...
+DUMP_MAX_NODES = 1 << 20   # ... and at most this many of them (in the engine's node order): 56 B a node, < 64 MB in all
+
+
+def dump_outputs(vol, out_dir):
+    """What the headline path (integrateBatchDevice) leaves behind after its last timed step: the fused volume, i.e. every
+    node's key (level, x, y, z), {sdf, weight}, split flag and colour, plus the last frame's counters.  The nodes are sampled
+    by a hash of their key, so two builds that disagree in some nodes still dump the same keys wherever they agree.
+    Under torchrun (N > 1) rank 0 calls it, so the dump is rank 0's shard of the volume."""
+    os.makedirs(out_dir, exist_ok=True)
+    d = vol.download_nodes()
+    k = d["keys"].astype(np.int64)
+    hsh = (k[:, 0] * 0x9E3779B1 ^ k[:, 1] * 0x85EBCA77 ^ k[:, 2] * 0xC2B2AE3D ^ k[:, 3] * 0x27D4EB2F) & 0xFFFFFFFF
+    sel = np.flatnonzero(hsh % DUMP_SAMPLE == 0)[:DUMP_MAX_NODES]
+    st = vol.stats()
+    arrays = {
+        "node_keys": d["keys"][sel].astype(np.float64),          # level, x, y, z (exact in float64)
+        "node_sdf_weight": d["dw"][sel].astype(np.float32),
+        "node_split": d["split"][sel].astype(np.float32),
+        "node_rgb": d["rgb"][sel].astype(np.float32),
+        "volume_counts": np.array([len(k), st.n_updates, st.n_node_visits, st.n_bricks, st.n_block_visits], np.float64),
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def workload_config(frames_per_step, n_gpus):
     return {"workload": "ICL-NUIM-shaped synthetic 640x480 stream (scene S2: 4 m room seen from inside, sigma(z) depth noise), "
                         "2048^3 voxels over 10 m, colour on (BASELINE.json configs[2] integrate leg)",
             "frames_per_step": frames_per_step, "image": [W, H], "grid": RES, "grid_size_m": SIZE,
             "point_bytes": 32, "distinct_frames": N_DISTINCT,
-            "l2": "inputs larger than L2 (64 distinct frames = 629 MB device-resident, orbit covers a >126 MB brick working set)",
+            "l2": "inputs larger than L2 (64 distinct frames = 629 MB device-resident, orbit covers a >50 MB brick working set)",
             "parallelism": "1 GPU" if n_gpus == 1 else f"volume sharded by coarse cell over {n_gpus} GPUs, every rank integrates every frame "
                            f"(end to end: each rank uploads 1/{n_gpus} of every frame, NVLink all-gather)"}
 
@@ -255,6 +282,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-host-load", action="store_true", help="skip the leg that repeats the device-resident measurement with all host cores busy")
     ap.add_argument("--pool-log2", type=int, default=18, help="brick pool capacity = 2^N slots (the bench scene allocates ~37k bricks)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the volume state of the headline leg's last step "
+                    "as DIR/<name>.npy (float32 / float64; a fixed sample of the nodes, see dump_outputs; rank 0's shard when N > 1)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -345,6 +374,8 @@ def main():
     vol.sync()
     prof, ms_total = timed(step_device, args.steps)
     nframes = args.steps * FRAMES_PER_STEP
+    if args.dump_outputs and rank == 0:
+        dump_outputs(vol, args.dump_outputs)
     value = nframes / (ms_total / 1e3)
 
     # ---- the same work one frame per call, the dominant kernel bracketed by CUDA events (roofline leg) ----
@@ -379,7 +410,7 @@ def main():
         with (HostLoad(os.cpu_count() or 1) if rank == 0 else contextlib.nullcontext()):
             step_device(k); k += FRAMES_PER_STEP
             vol.sync()
-            n_loaded = max(16, args.steps)
+            n_loaded = args.steps
             loaded = []
             for _ in range(3):                                 # three repeats: a descheduled submitting thread shows as an outlier, not as the figure
                 _, ms_loaded = timed(step_device, n_loaded)
@@ -411,13 +442,16 @@ def main():
     tp = os.path.join(ROOT, "profiles", "traffic.json")
     if world == 1 and os.path.exists(tp):
         try:
-            traffic = json.load(open(tp)).get("dram_bytes_per_launch")
+            cap = json.load(open(tp))
+            # a capture counts only for the GPU model it was taken on (tools/ncu_traffic.py records it)
+            if cap.get("device") == torch.cuda.get_device_name(local_rank):
+                traffic = cap.get("dram_bytes_per_launch")
         except Exception:
             traffic = None
     st_last = vol.stats()
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                 "traffic": traffic,
-                "traffic_source": "ncu --set full capture of this kernel on this workload at N=1 (profiles/traffic.json); not measured at N>1",
+                "traffic_source": f"profiles/traffic.json (a DRAM-counter capture of this kernel on this workload at N=1 on {cap['device']})" if traffic else "not measured",
                 "peak_source": peak_src, "kernel": "k_bricks (one warp per interior 8^3 block, brick updated in place)",
                 "bytes_per_launch": alg_bytes(prof_f) / max(1, prof_f.kernel_launches),
                 "us_per_launch": 1e3 * prof_f.ms_kernel / max(1, prof_f.kernel_launches),

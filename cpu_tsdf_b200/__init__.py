@@ -1,4 +1,4 @@
-"""cpu_tsdf_b200 — B200-native TSDF volumetric fusion, a drop-in for the volumetric path of
+"""cpu_tsdf_b200 — H100-native TSDF volumetric fusion, a drop-in for the volumetric path of
 sdmiller/cpu_tsdf.
 
 This package is the Python mirror of the reference's C++ class surface
@@ -171,7 +171,7 @@ class TSDFVolumeOctree:
         self._h = C.c_void_p()
         rc = self._lib.b200tsdf_create(C.byref(self._cfg), C.byref(self._h))
         if rc != 0:
-            raise B200Error({-2: "no CUDA device: the B200 engine has no CPU fallback"}.get(rc, f"b200tsdf_create failed ({rc})"))
+            raise B200Error({-2: "no CUDA device: the engine has no CPU fallback"}.get(rc, f"b200tsdf_create failed ({rc})"))
 
     def __del__(self):
         try:

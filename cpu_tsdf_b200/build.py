@@ -1,4 +1,4 @@
-"""In-tree build of libb200tsdf.so for sm_100a (nvcc cross-compiles without a GPU)."""
+"""In-tree build of libb200tsdf.so for sm_90a (H100; nvcc cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -16,7 +16,7 @@ SOURCES = {
 OBJ = os.path.join(CSRC, "_obj")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     # every float expression must round exactly as the reference's: no FMA contraction anywhere
     "-fmad=false", "-Xcompiler", "-fPIC,-ffp-contract=off,-O2",
     "-Xptxas", "-v",

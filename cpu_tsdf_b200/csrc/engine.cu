@@ -1,6 +1,6 @@
 // engine.cu — libb200tsdf.so: handle, device memory, kernels and the C ABI (include/b200tsdf.h).
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -fmad=false (see
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -fmad=false (see
 // __graft_entry__.build).  There is no CPU path: b200tsdf_create fails without a CUDA device.
 #include "../../include/b200tsdf.h"
 #include "tsdf_core.cuh"
@@ -410,9 +410,8 @@ __global__ void k_mesh_roots (Params gp, McParams mc, unsigned long long* __rest
 // ---------------------------------------------------------------------------------------------
 // ---- pinned staging for the host-packed uploads ---------------------------------------------------------------
 // The packing threads read the caller's points and write the staging while the copy engine reads the staging: when all of it
-// sits behind ONE socket's memory controllers that socket is the bottleneck (measured, tools/microbench/pack_numa.cu: 32 frames
-// packed + uploaded in 3.6 ms with input and staging on the same node, 3.1 ms = the PCIe time with the staging elsewhere or
-// interleaved).  The staging is therefore interleaved over the NUMA nodes (mbind; best effort — a refusal leaves default
+// sits behind ONE socket's memory controllers that socket can become the bottleneck (tools/microbench/pack_numa.cu compares
+// the placements).  The staging is therefore interleaved over the NUMA nodes (mbind; best effort — a refusal leaves default
 // placement) and then pinned with cudaHostRegister.
 struct Staging
 {
@@ -457,7 +456,7 @@ struct b200tsdf
   b200tsdf_config cfg_pending{}, cfg{};
   bool has_volume = false;
   Params p{};
-  int device = 0, sm_count = 148;
+  int device = 0, sm_count = 0;            // cudaDevAttrMultiProcessorCount, read in b200tsdf_create
   cudaStream_t stream = nullptr, copy_stream = nullptr, gather_stream = nullptr;   // compute | H2D uploads | pack + NVLink all-gather
   size_t pool = 0;
   bool alloc_color = false, alloc_var = false, alloc_norm = false;
@@ -856,7 +855,7 @@ int b200tsdf_reset (b200tsdf_t* h)
   CK (cudaMemsetAsync (p.keys, 0, pool * sizeof (uint64_t), s));
   CK (cudaMemsetAsync (p.split, 0, pool * BRICK_SPLIT_WORDS * sizeof (uint32_t), s));
   CK (cudaMemsetAsync (p.work, 0, pool, s));
-  k_fill_fresh<<<148 * 8, 256, 0, s>>> (p.nodes, pool * BRICK_NODES);
+  k_fill_fresh<<<h->sm_count * 8, 256, 0, s>>> (p.nodes, pool * BRICK_NODES);
   if (color) CK (cudaMemsetAsync (p.rgb, 0, pool * BRICK_NODES * sizeof (uchar4), s));
   if (var) { CK (cudaMemsetAsync (p.M, 0, pool * BRICK_NODES * sizeof (float), s)); CK (cudaMemsetAsync (p.ns, 0, pool * BRICK_NODES * sizeof (int), s)); }
   k_fill_fresh<<<64, 256, 0, s>>> (p.root_dw, root_n);
@@ -924,7 +923,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec& rec, const
     if (h->top_path)
     {
       // coarse levels above the supercells, top-down (none for 2048^3 / 10 m and 512^3 / 3 m)
-      for (int li = 0; li < h->nup; ++li) { k_upper_down<<<148 * 2, 128, 0, s>>> (p, d_rec, h->Q, li, 0, h->d_blist, h->d_stats); h->launches++; }
+      for (int li = 0; li < h->nup; ++li) { k_upper_down<<<h->sm_count * 2, 128, 0, s>>> (p, d_rec, h->Q, li, 0, h->d_blist, h->d_stats); h->launches++; }
       QNode* cells = h->super_static ? h->d_superq : h->Q.q[h->nup];
       const int qslot = h->super_static ? -1 : h->nup;
       auto kd = p.color ? k_celltop_down<true> : k_celltop_down<false>;
@@ -935,7 +934,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec& rec, const
     }
     else
     {
-      for (int li = 0; li < nl; ++li) { k_upper_down<<<148 * 2, 128, 0, s>>> (p, d_rec, h->Q, li, li == nl - 1, h->d_blist, h->d_stats); h->launches++; }
+      for (int li = 0; li < nl; ++li) { k_upper_down<<<h->sm_count * 2, 128, 0, s>>> (p, d_rec, h->Q, li, li == nl - 1, h->d_blist, h->d_stats); h->launches++; }
       bq = h->Q.q[nl - 1];
     }
     if (kr >= 0) CK (cudaEventRecord (h->kring[kr][0], s));
@@ -956,10 +955,10 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec& rec, const
       if (h->use_pdl) CK (launch_pdl (ku, dim3 (h->sm_count), dim3 (128), s, p, d_rec, cells, (const int*) h->d_count, (const QNode*) h->d_cellq, (const CellTop*) h->d_celltop, h->cell_cap, h->d_stats, h->sl, qslot, h->super_static));
       else ku<<<h->sm_count, 128, 0, s>>> (p, d_rec, cells, h->d_count, h->d_cellq, h->d_celltop, h->cell_cap, h->d_stats, h->sl, qslot, h->super_static);
       h->launches++;
-      for (int li = h->nup - 1; li >= 0; --li) { k_upper_up<<<148 * 2, 128, 0, s>>> (p, d_rec, h->Q, li, h->d_stats); h->launches++; }
+      for (int li = h->nup - 1; li >= 0; --li) { k_upper_up<<<h->sm_count * 2, 128, 0, s>>> (p, d_rec, h->Q, li, h->d_stats); h->launches++; }
     }
     else
-      for (int li = nl - 2; li >= 0; --li) { k_upper_up<<<148 * 2, 128, 0, s>>> (p, d_rec, h->Q, li, h->d_stats); h->launches++; }
+      for (int li = nl - 2; li >= 0; --li) { k_upper_up<<<h->sm_count * 2, 128, 0, s>>> (p, d_rec, h->Q, li, h->d_stats); h->launches++; }
   }
   else
   {

@@ -162,14 +162,13 @@ int b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows
   const size_t slice16 = (size_t) per * width * 16, frame16 = slice16 * nr;
   // host packing (host_pack.h): the caller's rows are packed to 16-byte pixels by host threads into pinned staging and only
   // those cross PCIe; without it the points are uploaded as they are (and packed on the device when there is a gather)
-  // The host packs at ~115 GB/s machine-wide whatever the number of ranks (measured, tools/microbench/pack_bench.cu), a PCIe link
-  // uploads raw points at ~48 GB/s PER RANK: packing on the host wins for one rank (8.0 k against 4.9 k frames/s), is a draw
-  // at two (6.4-7.7 k packed, 7.6 k raw) and loses from four on; with more than one rank the raw slices are therefore
-  // packed on the device.  B200TSDF_HOST_PACK=0 / 1 forces the choice.
+  // The host's packing rate is shared by all ranks of the machine (tools/microbench/pack_bench.cu measures it), while every
+  // rank has a PCIe link of its own: packing on the host halves the bytes one link carries and wins for one rank, but the
+  // shared packing rate falls behind the sum of the links as ranks are added; with more than one rank the raw slices are
+  // therefore packed on the device.  B200TSDF_HOST_PACK=0 / 1 forces the choice.
   const bool hpack = host_pack_wanted (h, stride, nr);
-  // frames per pipeline stage: with host packing short stages keep the copy engine right behind the packing threads (measured end
-  // to end on one GPU: 8 -> 6.4 k, 4 -> 7.4 k, 2 -> 7.9 k, 1 -> 8.0 k frames/s); a stage costs one NCCL launch when there is a
-  // gather, and device-side packing amortises its launches over 8
+  // frames per pipeline stage: with host packing short stages keep the copy engine right behind the packing threads; a stage
+  // costs one NCCL launch when there is a gather, and device-side packing amortises its launches over 8
   const int ROWS_CHUNK = h->rows_chunk > 0 ? h->rows_chunk : (hpack ? (nr == 1 ? 1 : 2) : 8);
   // two buffer sets, used alternately: set s is rewritten only after the batch that read it two calls ago has been fused
   const int s = h->rows_set;

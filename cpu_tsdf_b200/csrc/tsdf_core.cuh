@@ -1,4 +1,4 @@
-// tsdf_core.cuh — data layout and per-node arithmetic of the B200 TSDF engine.
+// tsdf_core.cuh — data layout and per-node arithmetic of the CUDA TSDF engine.
 //
 // The reference keeps the volume as a pointer-based octree of heap nodes
 // (include/cpu_tsdf/octree.h:55-172).  Here the same information — every node's {d,w}, a

@@ -1,4 +1,4 @@
-// b200_integrate — the reference's `integrate` program (src/prog/integrate.cpp) on the B200 engine.
+// b200_integrate — the reference's `integrate` program (src/prog/integrate.cpp) on the CUDA engine.
 //
 //   b200_integrate --in <dir> --out <dir> [options]          (same options as the reference, see --help)
 //
@@ -122,7 +122,7 @@ int main (int argc, char** argv)
     usage (argv[0]);
     return 1;
   }
-  if (opts.has ("cloud-only") || opts.has ("visualize")) { std::fprintf (stderr, "--cloud-only / --visualize are not supported by the B200 front end\n"); return 2; }
+  if (opts.has ("cloud-only") || opts.has ("visualize")) { std::fprintf (stderr, "--cloud-only / --visualize are not supported by this front end\n"); return 2; }
   const bool verbose = opts.has ("verbose"), flatten = opts.has ("flatten"), cleanup = opts.has ("cleanup"), invert = opts.has ("invert");
   const bool organized = opts.has ("organized"), world_frame = opts.has ("world"), zero_nans = opts.has ("zero-nans");
   const bool save_ascii = opts.has ("save-ascii"), save_tsdf = opts.has ("save-tsdf"), integrate_color = opts.has ("color");

@@ -1,4 +1,4 @@
-// pcd_io.h — PCD (Point Cloud Data v0.7) reader/writer for the front end of the B200 `integrate` program.
+// pcd_io.h — PCD (Point Cloud Data v0.7) reader/writer for the front end of the `b200_integrate` program.
 //
 // The reference loads its inputs with pcl::io::loadPCDFile into pcl::PointXYZRGBA (src/prog/integrate.cpp:548).
 // PCL is not a dependency here; this reads the three DATA encodings PCL writes (ascii, binary,

@@ -1,4 +1,4 @@
-// pose_io.h — camera poses of the B200 `integrate` program: the file formats and the Affine3d arithmetic of
+// pose_io.h — camera poses of the `b200_integrate` program: the file formats and the Affine3d arithmetic of
 // src/prog/integrate.cpp:452-483, 570, 638.  Eigen is not a dependency; the evaluation orders below restate
 // Eigen's [recalled]: Transform::inverse (Affine) = cofactor inverse of the linear part, t' = -(inv * t);
 // Transform * Transform (both Affine) = linear * linear, linear * t_rhs + t_lhs; 3-term sums as a0 + (a1 + a2).

@@ -1,4 +1,4 @@
-/* b200tsdf.h — C ABI of the B200-native TSDF fusion engine (libb200tsdf.so).
+/* b200tsdf.h — C ABI of the H100-native TSDF fusion engine (libb200tsdf.so).
  *
  * Drop-in boundary for the volumetric path of sdmiller/cpu_tsdf.  The reference has no FFI
  * layer: its boundary is the C++ class surface cpu_tsdf::TSDFVolumeOctree /

@@ -1,6 +1,8 @@
 """Shared helpers for the parity tests."""
 from __future__ import annotations
 
+import hashlib
+
 import numpy as np
 
 from cpu_tsdf_b200 import synth
@@ -40,6 +42,24 @@ def canon_soup(verts, cols=None):
     if len(t) == 0:
         return t
     return t[np.lexsort(t.T[::-1])]
+
+
+def digests(outputs):
+    """{name: array | bytes | number} -> {name: SHA-256 of the exact bytes, or the number itself}: the form in which outputs of
+    the reference's own sources are stored under tests/golden/ (tools/make_ref_pins.py)."""
+    out = {}
+    for k, v in outputs.items():
+        if isinstance(v, (bool, int, float, np.integer, np.floating)):
+            out[k] = v.item() if isinstance(v, np.generic) else v
+        else:
+            out[k] = hashlib.sha256(v if isinstance(v, bytes) else np.ascontiguousarray(v).tobytes()).hexdigest()
+    return out
+
+
+def nan_fixed(a):
+    """The bytes of `a` with every NaN made the same (mask + values): digests of these compare like np.array_equal(equal_nan=True)"""
+    a = np.ascontiguousarray(a)
+    return np.isnan(a).tobytes() + np.nan_to_num(a, nan=0.0, posinf=np.inf, neginf=-np.inf).tobytes()
 
 
 def query_points(seed=1, n=4000, radius=0.35, extent=1.6):

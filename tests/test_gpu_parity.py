@@ -1,4 +1,4 @@
-"""CUDA engine (through the C ABI / Python mirror) vs the CPU oracle on a real B200.
+"""CUDA engine (through the C ABI / Python mirror) vs the CPU oracle on a real H100.
 
 Bar (north_star): per-voxel {sdf,weight} and mesh vertices within a stated float tolerance,
 renderView depth within 1e-4 m.  The engine reproduces the reference's arithmetic expression by

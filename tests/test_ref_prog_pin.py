@@ -1,15 +1,28 @@
 """Pins oracle/prog_oracle.cpp (the restatement of the reference's program-side functions) to the reference's OWN text of
 src/prog/integrate.cpp, compiled from the source where it lies (oracle/Makefile `refprog`: meshToFaceCloud, flattenVertices,
 cleanupMesh, reprojectPoint, lines 63-222; the per-cloud preparation + z-buffer re-organisation of main(), lines 559-635).
-Needs oracle/_ref/libcpu_tsdf_refprog.so, which only a container with /root/reference can build; the built file travels."""
+The restatement's outputs must reproduce the digests of that build's outputs stored in tests/golden/ref_pins.json
+(tools/make_ref_pins.py); where oracle/_ref/libcpu_tsdf_refprog.so is built, its live outputs must reproduce them as well."""
+import json
 import os
 
 import numpy as np
 import pytest
 
 from oracle import oracle_py
+from tests.common import digests
 
-pytestmark = pytest.mark.skipif(not os.path.exists(oracle_py.REFPROG_LIB), reason="oracle/_ref/libcpu_tsdf_refprog.so not built (needs /root/reference)")
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+PINS = json.load(open(os.path.join(ROOT, "tests", "golden", "ref_pins.json")))["ref_prog_pin"]
+
+
+def pinned(key, run):
+    """run("port") must reproduce the stored digests of run("reference"); returns the port's outputs"""
+    got = run("port")
+    assert digests(got) == PINS[key]
+    if os.path.exists(oracle_py.REFPROG_LIB):
+        assert digests(run("reference")) == PINS[key]
+    return got
 
 
 def _cloud(rng, n, spread=1.0):
@@ -39,11 +52,12 @@ def test_organise_block_matches_the_reference_text(seed, units, zero_nans, world
         a = 0.3 * seed
         tf = np.array([[np.cos(a), 0, np.sin(a), 0.1], [0, 1, 0, -0.05], [-np.sin(a), 0, np.cos(a), 0.2], [0, 0, 0, 1]], np.float64)
     kw = dict(rgba_off=16, cloud_units=units, zero_nans=zero_nans, world_to_camera=tf)
-    a, na = oracle_py.organize(pts, intr, W, H, kind="reference", **kw)
-    b, nb = oracle_py.organize(pts, intr, W, H, kind="port", **kw)
-    assert na == nb > 500
-    # x, y, z and the colour word; the padding float and the bytes after the colour are whatever the default point holds
-    assert np.array_equal(a.view(np.uint32)[..., :3], b.view(np.uint32)[..., :3]) and np.array_equal(a.view(np.uint32)[..., 4], b.view(np.uint32)[..., 4])
+
+    def run(kind):
+        a, na = oracle_py.organize(pts, intr, W, H, kind=kind, **kw)
+        # x, y, z and the colour word; the padding float and the bytes after the colour are whatever the default point holds
+        return {"filled": na, "xyz": a.view(np.uint32)[..., :3], "bgra": a.view(np.uint32)[..., 4]}
+    assert pinned(f"organise_{seed}", run)["filled"] > 500
 
 
 def _mc_like_mesh(rng, n_quads, jitter):
@@ -70,10 +84,12 @@ def _mc_like_mesh(rng, n_quads, jitter):
 def test_flatten_vertices_matches_the_reference_text(seed, jitter, min_dist):
     rng = np.random.default_rng(seed)
     v, t = _mc_like_mesh(rng, 900, jitter)
-    va, ta = oracle_py.flatten_vertices(v, t, min_dist, kind="reference")
-    vb, tb = oracle_py.flatten_vertices(v, t, min_dist, kind="port")
-    assert len(va) == len(vb) and len(ta) == len(tb) and (min_dist == 0.0 or len(va) < len(v))
-    assert np.array_equal(va.view(np.uint32), vb.view(np.uint32)) and np.array_equal(ta, tb)
+
+    def run(kind):
+        va, ta = oracle_py.flatten_vertices(v, t, min_dist, kind=kind)
+        return {"n_verts": len(va), "n_tris": len(ta), "verts": va.view(np.uint32), "tris": ta}
+    out = pinned(f"flatten_{seed}", run)
+    assert min_dist == 0.0 or out["n_verts"] < len(v)
 
 
 @pytest.mark.parametrize("seed,face_dist,min_neighbors", [(1, 0.02, 5), (2, 0.008, 3), (3, 0.05, 40)])
@@ -81,7 +97,8 @@ def test_cleanup_mesh_matches_the_reference_text(seed, face_dist, min_neighbors)
     rng = np.random.default_rng(seed)
     v, t = _mc_like_mesh(rng, 400, 0.0)
     v, t = oracle_py.flatten_vertices(v, t, 1e-4, kind="port")       # cleanupMesh runs on the welded mesh in the program (:707-712)
-    va, ta = oracle_py.cleanup_mesh(v, t, face_dist, min_neighbors, kind="reference")
-    vb, tb = oracle_py.cleanup_mesh(v, t, face_dist, min_neighbors, kind="port")
-    assert len(ta) == len(tb) < len(t)
-    assert np.array_equal(va.view(np.uint32), vb.view(np.uint32)) and np.array_equal(ta, tb)
+
+    def run(kind):
+        va, ta = oracle_py.cleanup_mesh(v, t, face_dist, min_neighbors, kind=kind)
+        return {"n_tris": len(ta), "verts": va.view(np.uint32), "tris": ta}
+    assert pinned(f"cleanup_{seed}", run)["n_tris"] < len(t)
