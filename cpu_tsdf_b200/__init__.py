@@ -74,6 +74,7 @@ EXPORTS = [
     "b200tsdf_integrate_device", "b200tsdf_integrate_batch_device", "b200tsdf_integrate_async",
     "b200tsdf_comm_unique_id", "b200tsdf_comm_init", "b200tsdf_row_slice", "b200tsdf_integrate_batch_rows", "b200tsdf_gather_volume", "b200tsdf_sync", "b200tsdf_organize", "b200tsdf_integrate_unorganized", "b200tsdf_query", "b200tsdf_interpolate", "b200tsdf_render", "b200tsdf_mesh",
     "b200tsdf_free", "b200tsdf_save", "b200tsdf_load", "b200tsdf_export_shard", "b200tsdf_import_shard", "b200tsdf_voxel_center", "b200tsdf_voxel_index",
+    "b200tsdf_voxel_centers", "b200tsdf_occupied_voxel_indices", "b200tsdf_is_empty",
     "b200tsdf_get_stats", "b200tsdf_download_nodes", "b200tsdf_download_color_payload", "b200tsdf_frustum_cull",
     "b200tsdf_profile_begin", "b200tsdf_profile_end",
     "b200tsdf_mesh_flatten", "b200tsdf_mesh_cleanup", "b200tsdf_mesh_free", "b200tsdf_meshpost_last_error", "b200tsdf_debug_timing",
@@ -127,6 +128,9 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_import_shard.argtypes = [vp, vp, C.c_size_t]
     lib.b200tsdf_voxel_center.argtypes = [vp, C.c_int64, C.c_int64, C.c_int64, vp]
     lib.b200tsdf_voxel_index.argtypes = [vp, C.c_float, C.c_float, C.c_float, vp, vp]
+    lib.b200tsdf_voxel_centers.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(C.c_size_t)]
+    lib.b200tsdf_occupied_voxel_indices.argtypes = [vp, C.POINTER(vp), C.POINTER(C.c_size_t)]
+    lib.b200tsdf_is_empty.argtypes = [vp, C.POINTER(C.c_int32)]
     lib.b200tsdf_get_stats.argtypes = [vp, C.POINTER(Stats)]
     lib.b200tsdf_download_nodes.argtypes = [vp, vp, vp, vp, vp, vp, vp]; lib.b200tsdf_download_nodes.restype = C.c_int64
     lib.b200tsdf_download_color_payload.argtypes = [vp, vp]; lib.b200tsdf_download_color_payload.restype = C.c_int64
@@ -452,6 +456,35 @@ class TSDFVolumeOctree:
         o = np.empty(3, np.int32); ins = np.zeros(1, np.int32)
         self._check(self._lib.b200tsdf_voxel_index(self._h, x, y, z, _ptr(o), _ptr(ins)))
         return bool(ins[0]), o
+
+    def _leaf_records(self, buf, n, dtype):
+        out = np.empty((n, 3), dtype)
+        if n:
+            C.memmove(out.ctypes.data, buf.value, n * 12)
+        return out
+
+    def getVoxelCenters(self, nlevels: int = 4) -> np.ndarray:
+        """cpp:576-588 — centres of the nodes of Octree::getLeaves (nlevels) in the reference's depth-first order:
+        nlevels == 0 the root, < 0 every leaf, else every leaf above depth nlevels and every node at that depth.  [N, 3] float32."""
+        buf, n = C.c_void_p(), C.c_size_t()
+        self._check(self._lib.b200tsdf_voxel_centers(self._h, int(nlevels), C.byref(buf), C.byref(n)))
+        return self._leaf_records(buf, n.value, np.float32)
+
+    def getOccupiedVoxelIndices(self) -> np.ndarray:
+        """cpp:590-609 — getVoxelIndex of the centre of every leaf with w > 0 and |d| < 1, in leaf order.  [N, 3] int32."""
+        buf, n = C.c_void_p(), C.c_size_t()
+        self._check(self._lib.b200tsdf_occupied_voxel_indices(self._h, C.byref(buf), C.byref(n)))
+        return self._leaf_records(buf, n.value, np.int32)
+
+    def isEmpty(self) -> bool:
+        """tsdf_volume_octree.h:283-287 — True after reset(), False after any integrateCloud, the file's flag after load()."""
+        out = C.c_int32()
+        self._check(self._lib.b200tsdf_is_empty(self._h, C.byref(out)))
+        return bool(out.value)
+
+    def getIntensityCloud(self, trans=np.eye(4)):
+        """cpp:544-549 — an unimplemented stub in the reference that returns a null cloud; so does this."""
+        return None
 
     def getFrustumCulledVoxels(self, trans):
         """cpp:619-652 — returns the boolean mask over the 8^coarse cells."""

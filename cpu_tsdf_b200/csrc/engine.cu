@@ -403,6 +403,95 @@ __global__ void k_mesh_roots (Params gp, McParams mc, unsigned long long* __rest
   }
 }
 
+// ---- getLeaves (getVoxelCenters / getOccupiedVoxelIndices): the traversal of k_mesh_bricks / k_mesh_roots with
+// leaf_selected as predicate and one 12-byte record (centre or voxel index) plus its order key per selected node ----
+template <bool EMIT>
+__global__ void k_leaves_bricks (Params gp, const int* __restrict__ list, int nbricks, int nlevels, int occupied,
+                                 unsigned long long* __restrict__ total, unsigned long long* __restrict__ okeys, uint32_t* __restrict__ rec)
+{
+  B2_STAGE_PARAMS (gp)
+  int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  int lane = threadIdx.x & 31;
+  if (warp >= nbricks) return;
+  int slot = list[warp];
+  uint64_t key = p.keys[slot];
+  int t = (int) (key >> 60) - 1;
+  int bx = (int) ((key >> 40) & 0xFFFFF), by = (int) ((key >> 20) & 0xFFFFF), bz = (int) (key & 0xFFFFF);
+  int R = tier_root_level (p, t);
+  if (nlevels >= 0 && R + 1 > nlevels) return;                 // the whole brick lies below the depth limit
+  bool root_split = brick_root_is_split (p, t, bx, by, bz);
+  if (!root_split) return;                                     // nothing below an unsplit root exists
+  const uint32_t* sw = p.split + (size_t) slot * BRICK_SPLIT_WORDS;
+  for (int base = 0; base < BRICK_NODES; base += 32)
+  {
+    int i = base + lane;
+    BrickNode b{};
+    bool sel = false;
+    if (i < BRICK_NODES)
+    {
+      b = brick_node (p, sw, R, bx, by, bz, true, i);
+      float2 dw = make_float2 (-1.f, 0.f);
+      if (occupied) dw = p.nodes[(size_t) slot * BRICK_NODES + i];
+      sel = leaf_selected (b.level, b.exists, b.split, nlevels, occupied != 0, dw.x, dw.y);
+    }
+    // warp-scan compaction: ballot + popcount, one atomic per warp
+    const unsigned m = __ballot_sync (0xffffffffu, sel);
+    if (!m) continue;
+    unsigned long long wbase = 0;
+    if (lane == 0) wbase = atomicAdd (total, (unsigned long long) __popc (m));
+    wbase = __shfl_sync (0xffffffffu, wbase, 0);
+    if (EMIT && sel)
+    {
+      const size_t o = (size_t) wbase + __popc (m & ((1u << lane) - 1u));
+      NodePos n; n.level = b.level; n.x = b.x; n.y = b.y; n.z = b.z;
+      okeys[o] = mc_order_key (p, n);
+      leaf_record (p, b.level, b.x, b.y, b.z, occupied != 0, rec + 3 * o);
+    }
+  }
+}
+
+// root-array entries (coarse cells when Rtop == C; above the coarse depth they always have children)
+template <bool EMIT>
+__global__ void k_leaves_roots (Params gp, int nlevels, int occupied, unsigned long long* __restrict__ total,
+                                unsigned long long* __restrict__ okeys, uint32_t* __restrict__ rec)
+{
+  B2_STAGE_PARAMS (gp)
+  const int n = 1 << p.Rtop, lane = threadIdx.x & 31;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int z = i % n, y = (i / n) % n, x = i / (n * n);
+  NodePos nd{};
+  bool sel = false;
+  if (i < n * n * n)
+  {
+    nd = make_root (p, x, y, z);
+    const float2 dw = p.root_dw[nd.idx];
+    sel = leaf_selected (p.Rtop, true, is_split (p, nd), nlevels, occupied != 0, dw.x, dw.y);
+  }
+  // ballot compaction, one atomic per warp (the block size is a multiple of 32, so every lane reaches the ballot)
+  const unsigned m = __ballot_sync (0xffffffffu, sel);
+  if (!m) return;
+  unsigned long long wbase = 0;
+  if (lane == 0) wbase = atomicAdd (total, (unsigned long long) __popc (m));
+  wbase = __shfl_sync (0xffffffffu, wbase, 0);
+  if (EMIT && sel)
+  {
+    const size_t o = (size_t) wbase + __popc (m & ((1u << lane) - 1u));
+    okeys[o] = mc_order_key (p, nd);
+    leaf_record (p, p.Rtop, x, y, z, occupied != 0, rec + 3 * o);
+  }
+}
+
+// getLeaves (nlevels) for 0 <= nlevels < C (or nlevels == 0): every node of that depth, written straight into place
+__global__ void k_leaves_level (Params gp, int level, unsigned long long count, uint32_t* __restrict__ rec)
+{
+  B2_STAGE_PARAMS (gp)
+  unsigned long long i = (unsigned long long) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= count) return;
+  int x, y, z;
+  morton_decode (level, i, x, y, z);
+  leaf_record (p, level, x, y, z, false, rec + 3 * i);
+}
+
 } // namespace
 
 // ---------------------------------------------------------------------------------------------
@@ -532,6 +621,7 @@ struct b200tsdf
   }
   std::string err;
   float* mesh_v = nullptr; unsigned char* mesh_c = nullptr;
+  float* leaf_xyz = nullptr; int32_t* leaf_ijk = nullptr;   // b200tsdf_voxel_centers / _occupied_voxel_indices results
   // grow-only device scratch for the read-side calls (queries, render): no allocation per call
   unsigned char* d_scratch = nullptr; size_t scratch_cap = 0;
   int scratch (size_t bytes)
@@ -709,7 +799,7 @@ void b200tsdf_destroy (b200tsdf_t* h)
   if (h->stream) cudaStreamDestroy (h->stream);
   if (h->copy_stream) cudaStreamDestroy (h->copy_stream);
   if (h->gather_stream) cudaStreamDestroy (h->gather_stream);
-  std::free (h->mesh_v); std::free (h->mesh_c);
+  std::free (h->mesh_v); std::free (h->mesh_c); std::free (h->leaf_xyz); std::free (h->leaf_ijk);
   delete h;
 }
 
@@ -1475,7 +1565,7 @@ int b200tsdf_mesh (b200tsdf_t* h, float w_min, int color_mode, float** verts, ui
     CK (cudaMemsetAsync (d_total, 0, sizeof (unsigned long long), s));
     if (nb) k_mesh_bricks<true><<<(nb * 32 + 127) / 128, 128, 0, s>>> (p, mc, d_list, nb, d_total, d_v, d_c, d_k);
     k_mesh_roots<true><<<(root_n + 127) / 128, 128, 0, s>>> (p, mc, d_total, d_v, d_c, d_k);
-    if (b2_sort_triangles (s, (size_t) ntri, 3 * p.L + 3, d_k, d_v, d_c, d_v2, d_c2) != 0)
+    if (b2_sort_records (s, (size_t) ntri, 3 * p.L + 3, d_k, 9, d_v, d_c, d_v2, d_c2) != 0)
     { cudaFree (d_v); cudaFree (d_v2); cudaFree (d_c); cudaFree (d_c2); cudaFree (d_k); cudaFree (d_list); return h->fail (B200TSDF_ECUDA, "triangle sort failed"); }
     h->mesh_v = (float*) std::malloc (ntri * 9 * sizeof (float));
     CK (cudaMemcpyAsync (h->mesh_v, d_v2, ntri * 9 * sizeof (float), cudaMemcpyDeviceToHost, s));
@@ -1523,6 +1613,128 @@ int b200tsdf_frustum_cull (b200tsdf_t* h, const double* pose, uint8_t* mask, int
   CK (cudaStreamSynchronize (h->stream));
   cudaFree (d_mask);
   if (kept) { int k = 0; for (int i = 0; i < ncells; ++i) k += mask[i]; *kept = k; }
+  return B200TSDF_OK;
+}
+
+} // extern "C"
+
+namespace {
+
+// Octree::getLeaves (nlevels) on the device, one record per selected node (leaf_selected), in the reference's depth-first
+// order.  The records land in *out (3 x 32 bits each, malloc'ed, owned by the handle).  One enumeration: a counting pass,
+// then the emitting pass into buffers of exactly that size, a radix sort by order key and the copy to the host.  The brick
+// list lives in the handle's grow-only scratch (pool-sized, like the query buffers); the record and sort buffers are sized by
+// the result (hundreds of MB for a large volume) and are released before returning rather than kept on the handle.
+int enumerate_leaves (b200tsdf* h, int nlevels, bool occupied, const char* what, void** out, size_t* n)
+{
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, std::string (what) + " before reset()");
+  if (h->p.shard_count > 1)
+    return h->fail (B200TSDF_ESTATE, std::string (what) + " on a shard: a shard keeps the coarse cells it does not own as unsplit leaves; "
+                    "enumerate on the replica built by b200tsdf_gather_volume");
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  std::free (*out); *out = nullptr; *n = 0;
+  const Params& p = h->p;
+  cudaStream_t s = h->stream;
+  uint32_t *d_rec = nullptr, *d_rec2 = nullptr; unsigned long long* d_k = nullptr;
+  auto release = [&] () { cudaStreamSynchronize (s); cudaFree (d_rec); cudaFree (d_rec2); cudaFree (d_k); };
+  auto nomem = [&] (const char* m) { release (); cudaGetLastError (); return h->fail (B200TSDF_ENOMEM, m); };
+  // CK that frees this call's device buffers on the way out
+#define LCK(call)                                                                                  \
+  do {                                                                                             \
+    cudaError_t e_ = (call);                                                                       \
+    if (e_ != cudaSuccess) { release (); return h->fail (B200TSDF_ECUDA, std::string (#call) + ": " + cudaGetErrorString (e_)); } \
+  } while (0)
+  unsigned long long count = 0;
+  uint32_t* d_sorted = nullptr;
+  if (!occupied && nlevels >= 0 && (nlevels < p.C || nlevels == 0))
+  {
+    // every node of that depth exists (Octree::init) and none is ever pruned: 8^nlevels records, already in order
+    count = 1ull << (3 * nlevels);
+    if (cudaMalloc (&d_rec, count * 12) != cudaSuccess) return nomem ("device allocation failed (voxel centres)");
+    k_leaves_level<<<(unsigned) ((count + 127) / 128), 128, 0, s>>> (p, nlevels, count, d_rec);
+    d_sorted = d_rec;
+  }
+  else
+  {
+    int* d_nb = h->d_count + 40;
+    unsigned long long* d_total = h->d_stats + ST_SCRATCH;
+    if (int rc = h->scratch (h->pool * sizeof (int))) return rc;
+    int* d_list = (int*) h->d_scratch;
+    LCK (cudaMemsetAsync (d_nb, 0, sizeof (int), s));
+    LCK (cudaMemsetAsync (d_total, 0, sizeof (unsigned long long), s));
+    k_list_bricks<<<(unsigned) ((h->pool + 255) / 256), 256, 0, s>>> (p, d_list, d_nb);
+    int nb = 0;
+    LCK (cudaMemcpyAsync (&nb, d_nb, sizeof (int), cudaMemcpyDeviceToHost, s));
+    LCK (cudaStreamSynchronize (s));
+    const int root_n = (int) h->root_n, occ = occupied ? 1 : 0;
+    const unsigned bgrid = (unsigned) (((size_t) nb * 32 + 127) / 128), rgrid = (unsigned) ((root_n + 127) / 128);
+    if (nb) k_leaves_bricks<false><<<bgrid, 128, 0, s>>> (p, d_list, nb, nlevels, occ, d_total, nullptr, nullptr);
+    k_leaves_roots<false><<<rgrid, 128, 0, s>>> (p, nlevels, occ, d_total, nullptr, nullptr);
+    LCK (cudaMemcpyAsync (&count, d_total, sizeof (count), cudaMemcpyDeviceToHost, s));
+    LCK (cudaStreamSynchronize (s));
+    if (count)
+    {
+      if (cudaMalloc (&d_rec, count * 12) != cudaSuccess || cudaMalloc (&d_rec2, count * 12) != cudaSuccess
+          || cudaMalloc (&d_k, count * sizeof (unsigned long long)) != cudaSuccess)
+        return nomem ("device allocation failed (leaf records)");
+      LCK (cudaMemsetAsync (d_total, 0, sizeof (unsigned long long), s));
+      if (nb) k_leaves_bricks<true><<<bgrid, 128, 0, s>>> (p, d_list, nb, nlevels, occ, d_total, d_k, d_rec);
+      k_leaves_roots<true><<<rgrid, 128, 0, s>>> (p, nlevels, occ, d_total, d_k, d_rec);
+      // emission order depends on the hash layout and on atomics: sort into depth-first order
+      const int e = b2_sort_records (s, (size_t) count, 3 * p.L, d_k, 3, d_rec, nullptr, d_rec2, nullptr);
+      if (e == (int) cudaErrorMemoryAllocation) return nomem ("device allocation failed (leaf sort)");
+      if (e) { release (); return h->fail (B200TSDF_ECUDA, std::string ("leaf sort: ") + cudaGetErrorString ((cudaError_t) e)); }
+      d_sorted = d_rec2;
+    }
+  }
+#undef LCK
+  void* host = std::malloc (std::max<size_t> ((size_t) count, 1) * 12);
+  if (!host) return nomem ("host allocation failed (leaf records)");
+  cudaError_t e = cudaSuccess;
+  if (count) e = cudaMemcpyAsync (host, d_sorted, count * 12, cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize (s);
+  if (e == cudaSuccess) e = cudaGetLastError ();
+  release ();
+  if (e != cudaSuccess) { std::free (host); return h->fail (B200TSDF_ECUDA, std::string (what) + ": " + cudaGetErrorString (e)); }
+  h->d2h_bytes += (long long) (count * 12);
+  *out = host; *n = (size_t) count;
+  return check_device_err (h);
+}
+
+} // namespace
+
+extern "C" {
+
+int b200tsdf_voxel_centers (b200tsdf_t* h, int nlevels, float** xyz, size_t* n)
+{
+  if (!h || !xyz || !n) return B200TSDF_EINVAL;
+  *xyz = nullptr; *n = 0;
+  void* buf = h->leaf_xyz;
+  int rc = enumerate_leaves (h, nlevels, false, "getVoxelCenters", &buf, n);
+  h->leaf_xyz = (float*) buf;
+  if (rc) { *n = 0; return rc; }
+  *xyz = h->leaf_xyz;
+  return B200TSDF_OK;
+}
+
+int b200tsdf_occupied_voxel_indices (b200tsdf_t* h, int32_t** ijk, size_t* n)
+{
+  if (!h || !ijk || !n) return B200TSDF_EINVAL;
+  *ijk = nullptr; *n = 0;
+  void* buf = h->leaf_ijk;
+  int rc = enumerate_leaves (h, -1, true, "getOccupiedVoxelIndices", &buf, n);
+  h->leaf_ijk = (int32_t*) buf;
+  if (rc) { *n = 0; return rc; }
+  *ijk = h->leaf_ijk;
+  return B200TSDF_OK;
+}
+
+int b200tsdf_is_empty (b200tsdf_t* h, int32_t* out)
+{
+  if (!h || !out) return B200TSDF_EINVAL;
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "isEmpty before reset()");
+  *out = h->is_empty ? 1 : 0;
   return B200TSDF_OK;
 }
 

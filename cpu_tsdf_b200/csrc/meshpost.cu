@@ -340,25 +340,25 @@ extern "C" int b200tsdf_mesh_cleanup (int device, const float* verts, size_t nve
   return download_mesh (B, d_verts_out, nv_new, d_tris_out, nt_new, out_verts, out_nverts, out_tris, out_ntris);
 }
 
-// ---- triangle ordering for b200tsdf_mesh (engine.cu) -----------------------------------------------------------------
+// ---- record ordering for b200tsdf_mesh (triangles) and the leaf enumeration (engine.cu) ----------------------------------
 namespace {
-__global__ void k_gather_triangles (const unsigned int* __restrict__ order, size_t ntri, const float* __restrict__ v, const unsigned char* __restrict__ c,
-                                    float* __restrict__ vo, unsigned char* __restrict__ co)
+__global__ void k_gather_records (const unsigned int* __restrict__ order, size_t ntri, int words, const uint32_t* __restrict__ v,
+                                  const unsigned char* __restrict__ c, uint32_t* __restrict__ vo, unsigned char* __restrict__ co)
 {
-  // nine threads per triangle: thread q copies float q (and colour byte q) of the triangle
+  // `words` threads per record: thread q copies 32-bit word q (and colour byte q) of the record
   size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= ntri * 9) return;
-  size_t t = i / 9, q = i - t * 9, src = (size_t) order[t] * 9 + q;
+  if (i >= ntri * words) return;
+  size_t t = i / words, q = i - t * words, src = (size_t) order[t] * words + q;
   vo[i] = v[src];
   if (c) co[i] = c[src];
 }
 }
 
-int b2_sort_triangles (cudaStream_t s, size_t ntri, int key_bits, unsigned long long* d_keys, const float* d_v, const unsigned char* d_c,
-                       float* d_v_out, unsigned char* d_c_out)
+int b2_sort_records (cudaStream_t s, size_t ntri, int key_bits, unsigned long long* d_keys, int words, const void* d_v, const unsigned char* d_c,
+                     void* d_v_out, unsigned char* d_c_out)
 {
   if (!ntri) return 0;
-  if (ntri >= ((size_t) 1 << 31)) return (int) cudaErrorInvalidValue;
+  if (ntri >= ((size_t) 1 << 31) || words < 1) return (int) cudaErrorInvalidValue;
   unsigned long long* keys2 = nullptr; unsigned int *idx = nullptr, *idx2 = nullptr; void* tmp = nullptr;
   size_t bytes = 0;
   cudaError_t e = cudaMalloc (&keys2, ntri * 8);
@@ -368,7 +368,11 @@ int b2_sort_triangles (cudaStream_t s, size_t ntri, int key_bits, unsigned long 
   if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs (nullptr, bytes, d_keys, keys2, idx, idx2, (int) ntri, 0, key_bits, s);
   if (e == cudaSuccess) e = cudaMalloc (&tmp, bytes);
   if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs (tmp, bytes, d_keys, keys2, idx, idx2, (int) ntri, 0, key_bits, s);
-  if (e == cudaSuccess) { k_gather_triangles<<<nblk (ntri * 9), TPB, 0, s>>> (idx2, ntri, d_v, d_c, d_v_out, d_c_out); e = cudaGetLastError (); }
+  if (e == cudaSuccess)
+  {
+    k_gather_records<<<nblk (ntri * words), TPB, 0, s>>> (idx2, ntri, words, (const uint32_t*) d_v, d_c, (uint32_t*) d_v_out, d_c_out);
+    e = cudaGetLastError ();
+  }
   if (e == cudaSuccess) e = cudaStreamSynchronize (s);
   cudaFree (keys2); cudaFree (idx); cudaFree (idx2); cudaFree (tmp);
   return (int) e;

@@ -1176,6 +1176,73 @@ B2_HD unsigned long long mc_order_key (const Params& p, const NodePos& n)
   return k;
 }
 
+// ---- leaf enumeration: Octree::getLeaves (octree.cpp:99-109, :608-617) ----------------------------------
+// getLeaves (leaves, nlevels) walks depth first and emits a node of depth >= 1 when it has no children or its depth is
+// nlevels, never descending below nlevels (nlevels < 0: no limit).  The root is emitted only for nlevels == 0, which,
+// like every nlevels < C, is served apart: all nodes above the coarse depth exist by Octree::init.  `occupied` adds the
+// filter of getOccupiedVoxelIndices (tsdf_volume_octree.cpp:590-609): w > 0 && fabs (d) < 1.  The leaves of a call do
+// not overlap, so mc_order_key (of the node's first finest voxel) sorts them into the reference's order.
+B2_HD bool leaf_selected (int level, bool exists, bool has_children, int nlevels, bool occupied, float d, float w)
+{
+  if (!exists || level < 1) return false;
+  if (nlevels >= 0 && level > nlevels) return false;
+  if (has_children && level != nlevels) return false;
+  return !occupied || (w > 0.f && fabsf (d) < 1.f);
+}
+
+// node i (0..583) of the brick rooted at level R, coordinates (bx, by, bz): its level and coordinates, whether it exists
+// and whether it has children.  sw = the brick's split words, root_split = whether the brick's root has children.
+// Levels above the coarse depth always have children (Octree::init), whatever their storage says.
+struct BrickNode { int level, x, y, z; bool exists, split; };
+B2_HD BrickNode brick_node (const Params& p, const uint32_t* sw, int R, int bx, int by, int bz, bool root_split, int i)
+{
+  BrickNode b;
+  const int k = i < 8 ? 1 : (i < 72 ? 2 : 3);
+  const int j = i - node_offset (k);
+  b.level = R + k;
+  if (k == 1) b.exists = root_split;
+  else { const int pj = j >> 3; b.exists = b.level - 1 < p.C || ((sw[split_word_base (k - 1) + (pj >> 5)] >> (pj & 31)) & 1u); }
+  b.split = b.level < p.C || (b.level < p.L && ((sw[split_word_base (k) + (j >> 5)] >> (j & 31)) & 1u));
+  int lx = 0, ly = 0, lz = 0;
+  for (int q = k - 1; q >= 0; --q) { int c = (j >> (3 * q)) & 7; lx = (lx << 1) | (c >> 2); ly = (ly << 1) | ((c >> 1) & 1); lz = (lz << 1) | (c & 1); }
+  b.x = (bx << k) | lx; b.y = (by << k) | ly; b.z = (bz << k) | lz;
+  return b;
+}
+
+B2_HD uint32_t float_bits (float f)
+{
+#ifdef __CUDA_ARCH__
+  return __float_as_uint (f);
+#else
+  union { float f; uint32_t u; } c; c.f = f; return c.u;
+#endif
+}
+
+// the record of one selected node: its centre (OctreeNode::getCenter, the split-time accumulation) as three float bit
+// patterns, or getVoxelIndex of that centre (tsdf_volume_octree.cpp:562-574) as three int32
+B2_HD void leaf_record (const Params& p, int level, int x, int y, int z, bool index, uint32_t* o)
+{
+  const float cx = center1d (p, level, x), cy = center1d (p, level, y), cz = center1d (p, level, z);
+  if (index)
+  {
+    int xi, yi, zi;
+    voxel_index (p, cx, cy, cz, xi, yi, zi);
+    o[0] = (uint32_t) xi; o[1] = (uint32_t) yi; o[2] = (uint32_t) zi;
+  }
+  else { o[0] = float_bits (cx); o[1] = float_bits (cy); o[2] = float_bits (cz); }
+}
+
+// the i-th node of depth `level` in depth-first order (i's bits are the interleaved coordinates, x high)
+B2_HD void morton_decode (int level, unsigned long long i, int& x, int& y, int& z)
+{
+  x = y = z = 0;
+  for (int l = level - 1; l >= 0; --l)
+  {
+    const int c = (int) ((i >> (3 * l)) & 7);
+    x = (x << 1) | (c >> 2); y = (y << 1) | ((c >> 1) & 1); z = (z << 1) | (c & 1);
+  }
+}
+
 // getGridValue (cpp:91-106)
 B2_HD float mc_grid_value (const Params& p, const McParams& mc, int x, int y, int z)
 {

@@ -225,6 +225,22 @@ int  b200tsdf_gather_volume (b200tsdf_t* h, b200tsdf_t* full, int root);
 int  b200tsdf_voxel_center (const b200tsdf_t* h, int64_t x, int64_t y, int64_t z, float* out3);
 int  b200tsdf_voxel_index (const b200tsdf_t* h, float x, float y, float z, int32_t* out3, int32_t* inside);
 
+/* ---- leaf enumeration (Octree::getLeaves, octree.cpp:99-109, 608-617), in the reference's depth-first order ----
+ * Results are library-owned: valid until the next call of the same entry point or b200tsdf_destroy.  Both return
+ * B200TSDF_ESTATE before reset() and on a sharded handle (shard_count > 1: a shard keeps the coarse cells it does not
+ * own as unsplit leaves; enumerate on the replica of b200tsdf_gather_volume), B200TSDF_ENOMEM when the output or the
+ * sort buffers do not fit.
+ * TSDFVolumeOctree::getVoxelCenters (tsdf_volume_octree.cpp:576-588): the centres (OctreeNode::getCenter) of the nodes
+ * of getLeaves (nlevels) — nlevels == 0: the root; < 0: every leaf; else every leaf above depth nlevels and every node
+ * at depth nlevels.  *xyz = 3 floats per node. */
+int  b200tsdf_voxel_centers (b200tsdf_t* h, int nlevels, float** xyz, size_t* n);
+/* TSDFVolumeOctree::getOccupiedVoxelIndices (cpp:590-609): getVoxelIndex (cpp:562-574) of the centre of every leaf with
+ * w > 0 && |d| < 1.  *ijk = 3 int32 per leaf. */
+int  b200tsdf_occupied_voxel_indices (b200tsdf_t* h, int32_t** ijk, size_t* n);
+/* TSDFVolumeOctree::isEmpty (tsdf_volume_octree.h:283-287): 1 after reset(), 0 after any integrateCloud, the file's
+ * value after b200tsdf_load.  B200TSDF_ESTATE before reset(). */
+int  b200tsdf_is_empty (b200tsdf_t* h, int32_t* out);
+
 /* ---- introspection (tests, bench accounting) ------------------------------------------- */
 typedef struct b200tsdf_stats
 {

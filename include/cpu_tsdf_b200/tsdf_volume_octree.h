@@ -45,6 +45,7 @@ template <typename PointT> struct PointCloud
   bool is_dense = true;
   std::vector<PointT> points;
   typedef std::shared_ptr<PointCloud<PointT>> Ptr;
+  typedef std::shared_ptr<const PointCloud<PointT>> ConstPtr;
   const PointT& operator() (std::size_t column, std::size_t row) const { return points[row * width + column]; }
   std::size_t size () const { return points.size (); }
 };
@@ -54,6 +55,8 @@ struct Affine3d
   static Affine3d Identity () { return Affine3d (); }
   const double* data () const { return m; }
 };
+struct Intensity { float intensity = 0.f; };
+struct Vector3i { int x = 0, y = 0, z = 0; };              // stands in for Eigen::Vector3i in getOccupiedVoxelIndices
 struct TriangleSoup { std::vector<float> xyz; std::vector<std::uint8_t> rgb; std::vector<std::int32_t> polygons; };
 struct PointXYZRGBNormal { float x, y, z, pad = 1.f; float normal_x, normal_y, normal_z, npad = 0.f; std::uint8_t b = 0, g = 0, r = 0, a = 255; float curvature = 0.f, cpad[2] = { 0.f, 0.f }; };
 #else
@@ -61,7 +64,9 @@ using pcl::PointXYZRGBNormal;
 using pcl::PointCloud;
 using pcl::PointNormal;
 using pcl::PointXYZ;
+using pcl::Intensity;
 typedef Eigen::Affine3d Affine3d;
+typedef Eigen::Vector3i Vector3i;
 #endif
 
 namespace detail
@@ -80,6 +85,22 @@ inline void pose_rows (const Affine3d& t, double* m)
 #else
   std::memcpy (m, t.m, sizeof (double) * 16);
 #endif
+}
+inline Vector3i vector3i (const std::int32_t* v)
+{
+#ifdef B200TSDF_WITH_PCL
+  return Vector3i (v[0], v[1], v[2]);
+#else
+  Vector3i r; r.x = v[0]; r.y = v[1]; r.z = v[2]; return r;
+#endif
+}
+// OctreeNode::getCenter of the node with coordinate x at `level`: the split-time accumulation ctr -/+ size/4 from the
+// root at 0 (octree.cpp:244-266), as the engine replays it (tsdf_core.cuh center1d)
+inline float node_center1d (float size, int level, int x)
+{
+  float c = 0.f, off = size * 0.25f;
+  for (int i = level - 1; i >= 0; --i) { c = ((x >> i) & 1) ? c + off : c - off; off *= 0.5f; }
+  return c;
 }
 }
 
@@ -245,6 +266,69 @@ public:
   { float o[3] = { 0, 0, 0 }; b200tsdf_voxel_center (h_, (std::int64_t) x, (std::int64_t) y, (std::int64_t) z, o); PointXYZ p; p.x = o[0]; p.y = o[1]; p.z = o[2]; return p; }
   bool getVoxelIndex (float x, float y, float z, int& x_i, int& y_i, int& z_i) const               // cpp:562-574
   { std::int32_t o[3] = { 0, 0, 0 }, in = 0; b200tsdf_voxel_index (h_, x, y, z, o, &in); x_i = o[0]; y_i = o[1]; z_i = o[2]; return in != 0; }
+
+  // cpp:576-588: centres of the nodes of Octree::getLeaves (nlevels), depth first (nlevels == 0: the root; < 0: every leaf;
+  // else every leaf above depth nlevels and every node at depth nlevels).  Empty, with status () set, on failure.
+  typename PointCloud<PointXYZ>::ConstPtr getVoxelCenters (int nlevels = 4) const
+  {
+    typename PointCloud<PointXYZ>::Ptr cloud (new PointCloud<PointXYZ>);
+    float* v = nullptr; std::size_t n = 0;
+    status_ = h_ ? b200tsdf_voxel_centers (h_, nlevels, &v, &n) : B200TSDF_ENODEVICE;
+    if (status_ != 0) n = 0;
+    cloud->points.resize (n);
+    for (std::size_t i = 0; i < n; ++i) { cloud->points[i].x = v[3 * i]; cloud->points[i].y = v[3 * i + 1]; cloud->points[i].z = v[3 * i + 2]; }
+    cloud->width = static_cast<std::uint32_t> (n); cloud->height = 1;
+    return cloud;
+  }
+
+  // cpp:590-609: getVoxelIndex of the centre of every leaf with w > 0 && fabs (d) < 1, appended in leaf order
+  void getOccupiedVoxelIndices (std::vector<Vector3i>& indices) const
+  {
+    std::int32_t* v = nullptr; std::size_t n = 0;
+    status_ = h_ ? b200tsdf_occupied_voxel_indices (h_, &v, &n) : B200TSDF_ENODEVICE;
+    if (status_ != 0) return;
+    indices.reserve (indices.size () + n);
+    for (std::size_t i = 0; i < n; ++i) indices.push_back (detail::vector3i (v + 3 * i));
+  }
+
+  // h:283-287
+  bool isEmpty () const
+  {
+    std::int32_t e = 1;
+    status_ = h_ ? b200tsdf_is_empty (h_, &e) : B200TSDF_ENODEVICE;
+    return e != 0;
+  }
+
+  // cpp:544-549: a stub in the reference that returns a null cloud; so does this
+  typename PointCloud<Intensity>::Ptr getIntensityCloud (const Affine3d& /*trans*/ = Affine3d::Identity ()) const
+  { return typename PointCloud<Intensity>::Ptr (); }
+
+  // cpp:619-652.  The reference fills std::vector<OctreeNode::Ptr>; there are no node objects here (INTEGRATION.md §3), so
+  // this returns the centres of the culled coarse cells, in the reference's order (depth first over the coarse level),
+  // from the cull mask of b200tsdf_frustum_cull.
+  void getFrustumCulledVoxels (const Affine3d& trans, std::vector<PointXYZ>& centers) const
+  {
+    centers.clear ();
+    b200tsdf_stats st;
+    status_ = h_ ? b200tsdf_get_stats (h_, &st) : B200TSDF_ENODEVICE;
+    if (status_ != 0) return;
+    const int C = st.coarse_level, n = 1 << C;
+    std::vector<std::uint8_t> mask (static_cast<std::size_t> (n) * n * n);
+    double m[16];
+    detail::pose_rows (trans, m);
+    status_ = b200tsdf_frustum_cull (h_, m, mask.data (), nullptr);
+    if (status_ != 0) return;
+    for (std::size_t i = 0; i < mask.size (); ++i)                   // i = the bit-interleaved coordinates, x high
+    {
+      int x = 0, y = 0, z = 0;
+      for (int l = C - 1; l >= 0; --l)
+      { const int c = static_cast<int> ((i >> (3 * l)) & 7); x = (x << 1) | (c >> 2); y = (y << 1) | ((c >> 1) & 1); z = (z << 1) | (c & 1); }
+      if (!mask[(static_cast<std::size_t> (x) * n + y) * n + z]) continue;
+      PointXYZ p;
+      p.x = detail::node_center1d (cfg_.xsize, C, x); p.y = detail::node_center1d (cfg_.ysize, C, y); p.z = detail::node_center1d (cfg_.zsize, C, z);
+      centers.push_back (p);
+    }
+  }
 
   // TSDFInterface::instantiateFromFile (src/lib/tsdf_interface.cpp:44-51): "for now everything is an octree"
   static Ptr instantiateFromFile (const std::string& filename, int device = 0, int pool_log2 = 0)

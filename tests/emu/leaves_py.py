@@ -1,0 +1,63 @@
+"""ctypes wrapper of the host emulation of the leaf enumeration (tests/emu/leaves_emu.cpp, which compiles emu.cpp with
+emu_leaves added).  TEST HARNESS ONLY."""
+from __future__ import annotations
+
+import ctypes as C
+import os
+import subprocess
+
+import numpy as np
+
+from cpu_tsdf_b200 import Config
+from tests.emu import emu_py
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+LIB = os.path.join(HERE, "libemu_leaves.so")
+SRC = os.path.join(HERE, "leaves_emu.cpp")
+
+
+def build():
+    deps = [SRC, emu_py.SRC] + [os.path.join(emu_py.CORE, f) for f in ("tsdf_core.cuh", "organize.cuh", "meshpost_core.cuh", "host_math.h", "params_setup.h")]
+    if os.path.exists(LIB) and all(os.path.getmtime(LIB) >= os.path.getmtime(d) for d in deps):
+        return LIB
+    cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
+    subprocess.run([cxx, "-O2", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-x", "c++", SRC, "-o", LIB], check=True)
+    return LIB
+
+
+_lib = None
+
+
+def load():
+    global _lib
+    if _lib is None:
+        lib = C.CDLL(build())
+        vp = C.c_void_p
+        lib.emu_create.argtypes = [C.POINTER(Config)]; lib.emu_create.restype = vp
+        lib.emu_destroy.argtypes = [vp]
+        lib.emu_reset.argtypes = [vp]
+        lib.emu_integrate.argtypes = [vp, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, vp]
+        lib.emu_levels.argtypes = [vp, vp]
+        lib.emu_dump_nodes.argtypes = [vp] + [vp] * 6; lib.emu_dump_nodes.restype = C.c_longlong
+        lib.emu_leaves.argtypes = [vp, C.c_int, C.c_int, vp]; lib.emu_leaves.restype = C.c_longlong
+        _lib = lib
+    return _lib
+
+
+class EmuLeavesVolume(emu_py.EmuVolume):
+    """EmuVolume over the library that also has emu_leaves"""
+
+    def __init__(self, **kw):
+        lib = load()
+        saved = emu_py._lib
+        emu_py._lib = lib                      # EmuVolume.__init__ binds the library it loads
+        try:
+            super().__init__(**kw)
+        finally:
+            emu_py._lib = saved
+
+    def leaves(self, nlevels: int, occupied: bool = False) -> np.ndarray:
+        n = self.lib.emu_leaves(self.h, int(nlevels), int(occupied), None)
+        out = np.empty((n, 3), np.int32 if occupied else np.float32)
+        self.lib.emu_leaves(self.h, int(nlevels), int(occupied), out.ctypes.data_as(C.c_void_p))
+        return out
