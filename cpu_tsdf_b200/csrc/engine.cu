@@ -22,6 +22,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -36,6 +37,43 @@ using namespace b2;
 namespace {
 
 struct Planes { float pl[6][4]; };
+
+// A device buffer owned by one host call: freed when it goes out of scope, so error returns free it too.  Work queued on
+// its stream may still read it, so the stream is drained before the memory is released.
+template <typename T>
+struct DevBuf
+{
+  T* p = nullptr;
+  cudaStream_t s;
+  explicit DevBuf (cudaStream_t stream) : s (stream) {}
+  DevBuf (DevBuf&& o) noexcept : p (o.p), s (o.s) { o.p = nullptr; }
+  DevBuf& operator= (DevBuf&& o) noexcept { std::swap (p, o.p); std::swap (s, o.s); return *this; }
+  DevBuf (const DevBuf&) = delete;
+  DevBuf& operator= (const DevBuf&) = delete;
+  ~DevBuf () { release (); }
+  void release ()
+  {
+    if (!p) return;
+    cudaStreamSynchronize (s);
+    cudaFree (p);
+    p = nullptr;
+  }
+  cudaError_t alloc (size_t n)                  // n elements; n == 0 leaves the buffer null
+  {
+    release ();
+    if (!n) return cudaSuccess;
+    const cudaError_t e = cudaMalloc (&p, n * sizeof (T));
+    if (e != cudaSuccess) p = nullptr;
+    return e;
+  }
+  cudaError_t upload (const std::vector<T>& v)  // a device copy of v
+  {
+    cudaError_t e = alloc (v.size ());
+    if (e == cudaSuccess && !v.empty ()) e = cudaMemcpy (p, v.data (), v.size () * sizeof (T), cudaMemcpyHostToDevice);
+    return e;
+  }
+  operator T* () const { return p; }
+};
 
 // d_stats[0..ST_N) are cumulative since reset(); [ST_N..2*ST_N) is the snapshot taken at the start of
 // the current frame (so last-frame = cum - prev without a host round trip); the last slot is scratch
@@ -75,27 +113,14 @@ __global__ void k_build_superq (Params p, QNode* __restrict__ q, int n)
 }
 
 // frustum cull of the coarse cells (tsdf_volume_octree.cpp:619-652); planes come from the host
-__global__ void k_cull (Params p, Planes P, int* __restrict__ list, int* __restrict__ count, unsigned char* __restrict__ mask, QNode* __restrict__ q0)
+__global__ void k_cull (Params p, Planes P, unsigned char* __restrict__ mask)
 {
   int n = 1 << p.C;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n * n * n) return;
   int z = i % n, y = (i / n) % n, x = i / (n * n);
   float cx = center1d (p, p.C, x), cy = center1d (p, p.C, y), cz = center1d (p, p.C, z);
-  bool in = frustum_contains (P.pl, cx, cy, cz);
-  if (mask) mask[i] = in ? 1 : 0;
-  if (in && list && owns_cell (p, x, y, z))
-  {
-    int k = atomicAdd (count, 1);
-    list[k] = i;
-    if (q0)
-    {
-      NodePos n;
-      if (!locate_node (p, p.C, x, y, z, n)) { raise_err (p, ERR_MISSING_BRICK); n.slot = -1; n.idx = 0; }
-      QNode e; e.x = x; e.y = y; e.z = z; e.slot = n.slot; e.idx = n.idx; e.kind = KIND_DONE; e.child_base = -1; e.rc = 0;
-      q0[k] = e;
-    }
-  }
+  mask[i] = frustum_contains (P.pl, cx, cy, cz) ? 1 : 0;
 }
 
 // frame front end in ONE launch: blocks [0, cull_blocks) run the frustum cull of the coarse cells, the
@@ -280,8 +305,9 @@ __global__ void k_load_bricks (Params p, const uint64_t* __restrict__ keys, int 
   if (b >= n) return;
   if (threadIdx.x == 0)
   {
-    uint64_t key = keys[b];
-    slot_s = find_or_insert_brick (p, (int) (key >> 60) - 1, (int) ((key >> 40) & 0xFFFFF), (int) ((key >> 20) & 0xFFFFF), (int) (key & 0xFFFFF));
+    int t, bx, by, bz;
+    brick_key_decode (keys[b], t, bx, by, bz);
+    slot_s = find_or_insert_brick (p, t, bx, by, bz);
   }
   __syncthreads ();
   if (slot_s < 0) return;
@@ -308,74 +334,68 @@ __global__ void k_import_roots (Params p, int n, const int* __restrict__ idx, co
   if (p.root_M) { p.root_M[r] = M[i]; p.root_ns[r] = ns[i]; }
 }
 
-// ---- marching cubes: one warp per allocated brick, warp-scan compaction of the triangle soup ----
-__device__ __forceinline__ bool brick_root_is_split (const Params& p, int t, int bx, int by, int bz)
+// ---- the read-side walk of the flat layout (marching cubes, getLeaves): one warp per claimed brick whose root has children,
+// every node through brick_node, and one thread per root-array entry.  The emission order depends on the hash layout and on
+// atomics; the host sorts the records by order key afterwards. ----
+
+// exclusive prefix of the lanes' counts n and one atomicAdd on *total per warp: `first` = this lane's first output slot.
+// False when the whole warp has nothing to write.  Every lane of the warp must call it.
+__device__ __forceinline__ bool warp_reserve (unsigned long long* total, int n, unsigned long long& first)
 {
-  int R = tier_root_level (p, t);
-  if (R < p.C) return true;
-  NodePos r;
-  if (!locate_node (p, R, bx, by, bz, r)) return false;
-  return is_split (p, r);
+  const int lane = threadIdx.x & 31;
+  int incl = n;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync (0xffffffffu, incl, o); if (lane >= o) incl += v; }
+  const int wtotal = __shfl_sync (0xffffffffu, incl, 31);
+  if (wtotal == 0) return false;
+  unsigned long long wbase = 0;
+  if (lane == 0) wbase = atomicAdd (total, (unsigned long long) wtotal);
+  first = __shfl_sync (0xffffffffu, wbase, 0) + (unsigned long long) (incl - n);
+  return true;
 }
 
+// one cube's triangles from slot tri0 on, with their order keys (mc_order_key << 3 | triangle)
+__device__ __forceinline__ void mc_emit (const Params& p, const McParams& mc, const NodePos& n, float2 dw, int ntri, unsigned long long tri0,
+                                         float* verts, unsigned char* cols, unsigned long long* okeys)
+{
+  mc_leaf (p, mc, n, dw.x, dw.y, b200tsdf_mc::edge_table, b200tsdf_mc::tri_table, verts + tri0 * 9, cols ? cols + tri0 * 9 : nullptr);
+  const unsigned long long k = mc_order_key (p, n) << 3;
+  for (int t = 0; t < ntri; ++t) okeys[tri0 + t] = k | (unsigned long long) t;
+}
+
+// marching cubes: one cube per existing leaf at or below the coarse depth
 template <bool EMIT>
 __global__ void k_mesh_bricks (Params gp, McParams mc, const int* __restrict__ list, int nbricks,
                                unsigned long long* __restrict__ total, float* __restrict__ verts, unsigned char* __restrict__ cols,
                                unsigned long long* __restrict__ okeys)
 {
   B2_STAGE_PARAMS (gp)
-  int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  int lane = threadIdx.x & 31;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= nbricks) return;
-  int slot = list[warp];
-  uint64_t key = p.keys[slot];
-  int t = (int) (key >> 60) - 1;
-  int bx = (int) ((key >> 40) & 0xFFFFF), by = (int) ((key >> 20) & 0xFFFFF), bz = (int) (key & 0xFFFFF);
-  int R = tier_root_level (p, t);
-  bool root_split = brick_root_is_split (p, t, bx, by, bz);
-  if (!root_split) return;                                     // nothing below an unsplit root exists
+  const int slot = list[warp];
+  int t, bx, by, bz;
+  brick_key_decode (p.keys[slot], t, bx, by, bz);
+  if (!brick_root_is_split (p, t, bx, by, bz)) return;         // nothing below an unsplit root exists
+  const int R = tier_root_level (p, t);
   const uint32_t* sw = p.split + (size_t) slot * BRICK_SPLIT_WORDS;
   for (int base = 0; base < BRICK_NODES; base += 32)
   {
-    int i = base + lane;
+    const int i = base + lane;
     int ntri = 0;
-    NodePos n; float2 dw = make_float2 (-1.f, 0.f);
+    NodePos n; float2 dw;
     if (i < BRICK_NODES)
     {
-      int k = i < 8 ? 1 : (i < 72 ? 2 : 3);
-      int j = i - node_offset (k);
-      int level = R + k;
-      bool exists = true;
-      if (k > 1) { int pj = j >> 3; exists = (sw[split_word_base (k - 1) + (pj >> 5)] >> (pj & 31)) & 1; }
-      bool leaf = (level >= p.L) || !((sw[split_word_base (k) + (j >> 5)] >> (j & 31)) & 1);
-      if (exists && leaf && level >= p.C)
+      const BrickNode b = brick_node (p, sw, R, bx, by, bz, true, i);
+      if (b.exists && !b.split && b.level >= p.C)
       {
-        int lx = 0, ly = 0, lz = 0;
-        for (int q = k - 1; q >= 0; --q) { int c = (j >> (3 * q)) & 7; lx = (lx << 1) | (c >> 2); ly = (ly << 1) | ((c >> 1) & 1); lz = (lz << 1) | (c & 1); }
-        n.level = level; n.x = (bx << k) | lx; n.y = (by << k) | ly; n.z = (bz << k) | lz;
-        n.cx = center1d (p, level, n.x); n.cy = center1d (p, level, n.y); n.cz = center1d (p, level, n.z);
-        n.size = level_size (p, level); n.slot = slot; n.idx = i;
+        n = brick_node_pos (p, b, slot, i);
         dw = p.nodes[(size_t) slot * BRICK_NODES + i];
         ntri = mc_leaf (p, mc, n, dw.x, dw.y, b200tsdf_mc::edge_table, b200tsdf_mc::tri_table, nullptr, nullptr);
       }
     }
-    // warp-scan compaction: exclusive prefix of triangle counts, one atomic per warp
-    int incl = ntri;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { int v = __shfl_up_sync (0xffffffffu, incl, o); if (lane >= o) incl += v; }
-    int wtotal = __shfl_sync (0xffffffffu, incl, 31);
-    if (wtotal == 0) continue;
-    unsigned long long wbase = 0;
-    if (lane == 0) wbase = atomicAdd (total, (unsigned long long) wtotal);
-    wbase = __shfl_sync (0xffffffffu, wbase, 0);
-    if (EMIT && ntri > 0)
-    {
-      size_t tri0 = (size_t) wbase + (incl - ntri);
-      mc_leaf (p, mc, n, dw.x, dw.y, b200tsdf_mc::edge_table, b200tsdf_mc::tri_table,
-               verts + tri0 * 9, cols ? cols + tri0 * 9 : nullptr);
-      const unsigned long long k = mc_order_key (p, n) << 3;
-      for (int t = 0; t < ntri; ++t) okeys[tri0 + t] = k | (unsigned long long) t;
-    }
+    unsigned long long tri0;
+    if (!warp_reserve (total, ntri, tri0)) continue;
+    if (EMIT && ntri > 0) mc_emit (p, mc, n, dw, ntri, tri0, verts, cols, okeys);
   }
 }
 
@@ -385,46 +405,51 @@ __global__ void k_mesh_roots (Params gp, McParams mc, unsigned long long* __rest
                               unsigned long long* __restrict__ okeys)
 {
   B2_STAGE_PARAMS (gp)
-  int n = 1 << p.Rtop;
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n * n * n || p.Rtop < p.C) return;
-  int z = i % n, y = (i / n) % n, x = i / (n * n);
-  NodePos nd = make_root (p, x, y, z);
-  if (is_split (p, nd)) return;
-  float2 dw = p.root_dw[nd.idx];
-  int ntri = mc_leaf (p, mc, nd, dw.x, dw.y, b200tsdf_mc::edge_table, b200tsdf_mc::tri_table, nullptr, nullptr);
-  if (!ntri) return;
-  unsigned long long base = atomicAdd (total, (unsigned long long) ntri);
-  if (EMIT)
+  const int n = 1 << p.Rtop;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  int ntri = 0;
+  NodePos nd; float2 dw;
+  if (i < n * n * n)                                           // (the block size is a multiple of 32: every lane reaches warp_reserve)
   {
-    mc_leaf (p, mc, nd, dw.x, dw.y, b200tsdf_mc::edge_table, b200tsdf_mc::tri_table, verts + base * 9, cols ? cols + base * 9 : nullptr);
-    const unsigned long long k = mc_order_key (p, nd) << 3;
-    for (int t = 0; t < ntri; ++t) okeys[base + t] = k | (unsigned long long) t;
+    nd = make_root (p, i / (n * n), (i / n) % n, i % n);
+    if (!is_split (p, nd))
+    {
+      dw = p.root_dw[nd.idx];
+      ntri = mc_leaf (p, mc, nd, dw.x, dw.y, b200tsdf_mc::edge_table, b200tsdf_mc::tri_table, nullptr, nullptr);
+    }
   }
+  unsigned long long tri0;
+  if (!warp_reserve (total, ntri, tri0)) return;
+  if (EMIT && ntri > 0) mc_emit (p, mc, nd, dw, ntri, tri0, verts, cols, okeys);
 }
 
-// ---- getLeaves (getVoxelCenters / getOccupiedVoxelIndices): the traversal of k_mesh_bricks / k_mesh_roots with
-// leaf_selected as predicate and one 12-byte record (centre or voxel index) plus its order key per selected node ----
+// getLeaves (getVoxelCenters / getOccupiedVoxelIndices): leaf_selected as predicate and one 12-byte record (centre or voxel
+// index) plus its order key per selected node
+__device__ __forceinline__ void leaf_emit (const Params& p, int level, int x, int y, int z, bool index, unsigned long long o,
+                                           unsigned long long* okeys, uint32_t* rec)
+{
+  NodePos n; n.level = level; n.x = x; n.y = y; n.z = z;
+  okeys[o] = mc_order_key (p, n);
+  leaf_record (p, level, x, y, z, index, rec + 3 * o);
+}
+
 template <bool EMIT>
 __global__ void k_leaves_bricks (Params gp, const int* __restrict__ list, int nbricks, int nlevels, int occupied,
                                  unsigned long long* __restrict__ total, unsigned long long* __restrict__ okeys, uint32_t* __restrict__ rec)
 {
   B2_STAGE_PARAMS (gp)
-  int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  int lane = threadIdx.x & 31;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= nbricks) return;
-  int slot = list[warp];
-  uint64_t key = p.keys[slot];
-  int t = (int) (key >> 60) - 1;
-  int bx = (int) ((key >> 40) & 0xFFFFF), by = (int) ((key >> 20) & 0xFFFFF), bz = (int) (key & 0xFFFFF);
-  int R = tier_root_level (p, t);
+  const int slot = list[warp];
+  int t, bx, by, bz;
+  brick_key_decode (p.keys[slot], t, bx, by, bz);
+  const int R = tier_root_level (p, t);
   if (nlevels >= 0 && R + 1 > nlevels) return;                 // the whole brick lies below the depth limit
-  bool root_split = brick_root_is_split (p, t, bx, by, bz);
-  if (!root_split) return;                                     // nothing below an unsplit root exists
+  if (!brick_root_is_split (p, t, bx, by, bz)) return;         // nothing below an unsplit root exists
   const uint32_t* sw = p.split + (size_t) slot * BRICK_SPLIT_WORDS;
   for (int base = 0; base < BRICK_NODES; base += 32)
   {
-    int i = base + lane;
+    const int i = base + lane;
     BrickNode b{};
     bool sel = false;
     if (i < BRICK_NODES)
@@ -434,19 +459,9 @@ __global__ void k_leaves_bricks (Params gp, const int* __restrict__ list, int nb
       if (occupied) dw = p.nodes[(size_t) slot * BRICK_NODES + i];
       sel = leaf_selected (b.level, b.exists, b.split, nlevels, occupied != 0, dw.x, dw.y);
     }
-    // warp-scan compaction: ballot + popcount, one atomic per warp
-    const unsigned m = __ballot_sync (0xffffffffu, sel);
-    if (!m) continue;
-    unsigned long long wbase = 0;
-    if (lane == 0) wbase = atomicAdd (total, (unsigned long long) __popc (m));
-    wbase = __shfl_sync (0xffffffffu, wbase, 0);
-    if (EMIT && sel)
-    {
-      const size_t o = (size_t) wbase + __popc (m & ((1u << lane) - 1u));
-      NodePos n; n.level = b.level; n.x = b.x; n.y = b.y; n.z = b.z;
-      okeys[o] = mc_order_key (p, n);
-      leaf_record (p, b.level, b.x, b.y, b.z, occupied != 0, rec + 3 * o);
-    }
+    unsigned long long o;
+    if (!warp_reserve (total, sel ? 1 : 0, o)) continue;
+    if (EMIT && sel) leaf_emit (p, b.level, b.x, b.y, b.z, occupied != 0, o, okeys, rec);
   }
 }
 
@@ -456,29 +471,19 @@ __global__ void k_leaves_roots (Params gp, int nlevels, int occupied, unsigned l
                                 unsigned long long* __restrict__ okeys, uint32_t* __restrict__ rec)
 {
   B2_STAGE_PARAMS (gp)
-  const int n = 1 << p.Rtop, lane = threadIdx.x & 31;
+  const int n = 1 << p.Rtop;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int z = i % n, y = (i / n) % n, x = i / (n * n);
-  NodePos nd{};
   bool sel = false;
-  if (i < n * n * n)
+  if (i < n * n * n)                                           // (the block size is a multiple of 32: every lane reaches warp_reserve)
   {
-    nd = make_root (p, x, y, z);
+    const NodePos nd = make_root (p, x, y, z);
     const float2 dw = p.root_dw[nd.idx];
     sel = leaf_selected (p.Rtop, true, is_split (p, nd), nlevels, occupied != 0, dw.x, dw.y);
   }
-  // ballot compaction, one atomic per warp (the block size is a multiple of 32, so every lane reaches the ballot)
-  const unsigned m = __ballot_sync (0xffffffffu, sel);
-  if (!m) return;
-  unsigned long long wbase = 0;
-  if (lane == 0) wbase = atomicAdd (total, (unsigned long long) __popc (m));
-  wbase = __shfl_sync (0xffffffffu, wbase, 0);
-  if (EMIT && sel)
-  {
-    const size_t o = (size_t) wbase + __popc (m & ((1u << lane) - 1u));
-    okeys[o] = mc_order_key (p, nd);
-    leaf_record (p, p.Rtop, x, y, z, occupied != 0, rec + 3 * o);
-  }
+  unsigned long long o;
+  if (!warp_reserve (total, sel ? 1 : 0, o)) return;
+  if (EMIT && sel) leaf_emit (p, p.Rtop, x, y, z, occupied != 0, o, okeys, rec);
 }
 
 // getLeaves (nlevels) for 0 <= nlevels < C (or nlevels == 0): every node of that depth, written straight into place
@@ -620,8 +625,8 @@ struct b200tsdf
     }
   }
   std::string err;
-  float* mesh_v = nullptr; unsigned char* mesh_c = nullptr;
-  float* leaf_xyz = nullptr; int32_t* leaf_ijk = nullptr;   // b200tsdf_voxel_centers / _occupied_voxel_indices results
+  void* mesh_v = nullptr; void* mesh_c = nullptr;           // b200tsdf_mesh results (malloc'ed)
+  void* leaf_xyz = nullptr; void* leaf_ijk = nullptr;       // b200tsdf_voxel_centers / _occupied_voxel_indices results
   // grow-only device scratch for the read-side calls (queries, render): no allocation per call
   unsigned char* d_scratch = nullptr; size_t scratch_cap = 0;
   int scratch (size_t bytes)
@@ -703,6 +708,74 @@ void fill_frame (const b200tsdf* h, Frame& f, const unsigned char* d_pts, size_t
   double inv[12];
   b2host::affine_inverse (pose, inv);                                 // hpp:54: trans.inverse ().cast<float> ()
   for (int i = 0; i < 12; ++i) { f.tinv[i] = (float) inv[i]; f.tfwd[i] = (float) pose[i]; }
+}
+
+// The claimed brick slots, listed into the handle's grow-only scratch.  Returns their number, or a B200TSDF_ error (< 0).
+// The list lives until the next use of the scratch.
+int list_bricks (b200tsdf* h, int*& list)
+{
+  if (int rc = h->scratch (h->pool * sizeof (int))) return rc;
+  list = (int*) h->d_scratch;
+  int* d_n = h->d_count + 40;
+  cudaStream_t s = h->stream;
+  CK (cudaMemsetAsync (d_n, 0, sizeof (int), s));
+  k_list_bricks<<<(unsigned) ((h->pool + 255) / 256), 256, 0, s>>> (h->p, list, d_n);
+  int nb = 0;
+  CK (cudaMemcpyAsync (&nb, d_n, sizeof (int), cudaMemcpyDeviceToHost, s));
+  CK (cudaStreamSynchronize (s));
+  return nb;
+}
+
+// A failed device allocation is reported as B200TSDF_ENOMEM; the runtime's last error is cleared so that no later call
+// reports it.
+int alloc_failed (b200tsdf* h, const std::string& what)
+{
+  cudaGetLastError ();
+  return h->fail (B200TSDF_ENOMEM, "device allocation failed (" + what + ")");
+}
+
+// `bytes` of device memory into `host` (reallocated with malloc, at least one byte), after the work queued before them
+int download (b200tsdf* h, const void* d, size_t bytes, void*& host)
+{
+  std::free (host);
+  host = std::malloc (std::max<size_t> (bytes, 1));
+  if (!host) return h->fail (B200TSDF_ENOMEM, "host allocation failed");
+  if (bytes) CK (cudaMemcpyAsync (host, d, bytes, cudaMemcpyDeviceToHost, h->stream));
+  CK (cudaStreamSynchronize (h->stream));
+  CK (cudaGetLastError ());
+  return B200TSDF_OK;
+}
+
+// The enumeration behind marching cubes and getLeaves, in the reference's depth-first order.  launch (emit, total, keys, v, c)
+// enqueues the caller's kernels: with emit = std::false_type they add their record count to *total, with std::true_type they
+// also write their records at the slots they reserve, with the order key of each in keys.  A record is `words` 32-bit words
+// in v, plus `words` bytes in c when host_c is given.  The records are counted, emitted into device buffers of exactly that
+// size, sorted by the low key_bits of their keys and copied into host_v / *host_c (see download).  A failed allocation
+// returns B200TSDF_ENOMEM.
+template <typename Launch>
+int sorted_records (b200tsdf* h, const char* what, int words, int key_bits, const Launch& launch,
+                    void*& host_v, void** host_c, unsigned long long& count)
+{
+  cudaStream_t s = h->stream;
+  unsigned long long* d_total = h->d_stats + ST_SCRATCH;
+  count = 0;
+  CK (cudaMemsetAsync (d_total, 0, sizeof (count), s));
+  launch (std::false_type (), d_total, nullptr, nullptr, nullptr);
+  CK (cudaMemcpyAsync (&count, d_total, sizeof (count), cudaMemcpyDeviceToHost, s));
+  CK (cudaStreamSynchronize (s));
+  const size_t nw = (size_t) count * words, nc = host_c ? nw : 0;
+  DevBuf<uint32_t> v (s), v2 (s); DevBuf<unsigned char> c (s), c2 (s); DevBuf<unsigned long long> k (s);
+  if (count)
+  {
+    if (v.alloc (nw) || v2.alloc (nw) || c.alloc (nc) || c2.alloc (nc) || k.alloc (count)) return alloc_failed (h, what);
+    CK (cudaMemsetAsync (d_total, 0, sizeof (count), s));
+    launch (std::true_type (), d_total, k, v, c);
+    const int e = b2_sort_records (s, (size_t) count, key_bits, k, words, v, c, v2, c2);
+    if (e == (int) cudaErrorMemoryAllocation) return alloc_failed (h, std::string (what) + " sort");
+    if (e) return h->fail (B200TSDF_ECUDA, std::string (what) + " sort: " + cudaGetErrorString ((cudaError_t) e));
+  }
+  if (int rc = download (h, v2, nw * 4, host_v)) return rc;
+  return host_c ? download (h, c2, nc, *host_c) : B200TSDF_OK;
 }
 
 } // namespace
@@ -1537,44 +1610,22 @@ int b200tsdf_mesh (b200tsdf_t* h, float w_min, int color_mode, float** verts, ui
   McParams mc;
   make_mc_params (h->cfg, p, w_min, color_mode, mc);
   cudaStream_t s = h->stream;
-  int* d_list = nullptr; int* d_n = h->d_count + 40;
-  unsigned long long* d_total = h->d_stats + ST_SCRATCH;
-  CK (cudaMalloc (&d_list, h->pool * sizeof (int)));
-  CK (cudaMemsetAsync (d_n, 0, sizeof (int), s));
-  CK (cudaMemsetAsync (d_total, 0, sizeof (unsigned long long), s));
-  k_list_bricks<<<(unsigned) ((h->pool + 255) / 256), 256, 0, s>>> (p, d_list, d_n);
-  int nb = 0;
-  CK (cudaMemcpyAsync (&nb, d_n, sizeof (int), cudaMemcpyDeviceToHost, s));
-  CK (cudaStreamSynchronize (s));
-  int root_n = (int) h->root_n;
-  if (nb) k_mesh_bricks<false><<<(nb * 32 + 127) / 128, 128, 0, s>>> (p, mc, d_list, nb, d_total, nullptr, nullptr, nullptr);
-  k_mesh_roots<false><<<(root_n + 127) / 128, 128, 0, s>>> (p, mc, d_total, nullptr, nullptr, nullptr);
-  unsigned long long ntri = 0;
-  CK (cudaMemcpyAsync (&ntri, d_total, sizeof (ntri), cudaMemcpyDeviceToHost, s));
-  CK (cudaStreamSynchronize (s));
-  std::free (h->mesh_v); std::free (h->mesh_c); h->mesh_v = nullptr; h->mesh_c = nullptr;
-  *verts = nullptr; if (rgb) *rgb = nullptr; *nverts = (size_t) ntri * 3;
-  if (ntri)
+  int* list = nullptr;
+  const int nb = list_bricks (h, list);
+  if (nb < 0) return nb;
+  const unsigned bgrid = (unsigned) (((size_t) nb * 32 + 127) / 128), rgrid = (unsigned) ((h->root_n + 127) / 128);
+  auto launch = [&] (auto emit, unsigned long long* total, unsigned long long* keys, void* v, unsigned char* c)
   {
-    // emission order depends on the hash layout and on atomics; the triangles are then sorted into the reference's
-    // own order (depth first over the octree, mc_order_key) so that the soup is reproducible and comparable as is
-    float *d_v = nullptr, *d_v2 = nullptr; unsigned char *d_c = nullptr, *d_c2 = nullptr; unsigned long long* d_k = nullptr;
-    CK (cudaMalloc (&d_v, ntri * 9 * sizeof (float))); CK (cudaMalloc (&d_v2, ntri * 9 * sizeof (float)));
-    CK (cudaMalloc (&d_k, ntri * sizeof (unsigned long long)));
-    if (color_mode) { CK (cudaMalloc (&d_c, ntri * 9)); CK (cudaMalloc (&d_c2, ntri * 9)); }
-    CK (cudaMemsetAsync (d_total, 0, sizeof (unsigned long long), s));
-    if (nb) k_mesh_bricks<true><<<(nb * 32 + 127) / 128, 128, 0, s>>> (p, mc, d_list, nb, d_total, d_v, d_c, d_k);
-    k_mesh_roots<true><<<(root_n + 127) / 128, 128, 0, s>>> (p, mc, d_total, d_v, d_c, d_k);
-    if (b2_sort_records (s, (size_t) ntri, 3 * p.L + 3, d_k, 9, d_v, d_c, d_v2, d_c2) != 0)
-    { cudaFree (d_v); cudaFree (d_v2); cudaFree (d_c); cudaFree (d_c2); cudaFree (d_k); cudaFree (d_list); return h->fail (B200TSDF_ECUDA, "triangle sort failed"); }
-    h->mesh_v = (float*) std::malloc (ntri * 9 * sizeof (float));
-    CK (cudaMemcpyAsync (h->mesh_v, d_v2, ntri * 9 * sizeof (float), cudaMemcpyDeviceToHost, s));
-    if (color_mode) { h->mesh_c = (unsigned char*) std::malloc (ntri * 9); CK (cudaMemcpyAsync (h->mesh_c, d_c2, ntri * 9, cudaMemcpyDeviceToHost, s)); }
-    CK (cudaStreamSynchronize (s));
-    cudaFree (d_v); cudaFree (d_v2); cudaFree (d_c); cudaFree (d_c2); cudaFree (d_k);
-    *verts = h->mesh_v; if (rgb) *rgb = h->mesh_c;
-  }
-  cudaFree (d_list);
+    constexpr bool E = decltype (emit)::value;
+    if (nb) k_mesh_bricks<E><<<bgrid, 128, 0, s>>> (p, mc, list, nb, total, (float*) v, c, keys);
+    k_mesh_roots<E><<<rgrid, 128, 0, s>>> (p, mc, total, (float*) v, c, keys);
+  };
+  std::free (h->mesh_c); h->mesh_c = nullptr;
+  unsigned long long ntri = 0;
+  if (int rc = sorted_records (h, "triangles", 9, 3 * p.L + 3, launch, h->mesh_v, color_mode ? &h->mesh_c : nullptr, ntri)) return rc;
+  *nverts = (size_t) ntri * 3;
+  *verts = ntri ? (float*) h->mesh_v : nullptr;
+  if (rgb) *rgb = ntri ? (uint8_t*) h->mesh_c : nullptr;
   return check_device_err (h);
 }
 
@@ -1606,12 +1657,11 @@ int b200tsdf_frustum_cull (b200tsdf_t* h, const double* pose, uint8_t* mask, int
   Planes P;
   b2host::frustum_planes (pose, p.width, p.height, p.fx, p.fy, p.min_sensor, p.max_sensor, P.pl);
   int ncells = 1 << (3 * p.C);
-  unsigned char* d_mask = nullptr;
-  CK (cudaMalloc (&d_mask, ncells));
-  k_cull<<<(ncells + 127) / 128, 128, 0, h->stream>>> (p, P, nullptr, nullptr, d_mask, nullptr);
+  DevBuf<unsigned char> d_mask (h->stream);
+  CK (d_mask.alloc (ncells));
+  k_cull<<<(ncells + 127) / 128, 128, 0, h->stream>>> (p, P, d_mask);
   CK (cudaMemcpyAsync (mask, d_mask, ncells, cudaMemcpyDeviceToHost, h->stream));
   CK (cudaStreamSynchronize (h->stream));
-  cudaFree (d_mask);
   if (kept) { int k = 0; for (int i = 0; i < ncells; ++i) k += mask[i]; *kept = k; }
   return B200TSDF_OK;
 }
@@ -1621,11 +1671,10 @@ int b200tsdf_frustum_cull (b200tsdf_t* h, const double* pose, uint8_t* mask, int
 namespace {
 
 // Octree::getLeaves (nlevels) on the device, one record per selected node (leaf_selected), in the reference's depth-first
-// order.  The records land in *out (3 x 32 bits each, malloc'ed, owned by the handle).  One enumeration: a counting pass,
-// then the emitting pass into buffers of exactly that size, a radix sort by order key and the copy to the host.  The brick
-// list lives in the handle's grow-only scratch (pool-sized, like the query buffers); the record and sort buffers are sized by
-// the result (hundreds of MB for a large volume) and are released before returning rather than kept on the handle.
-int enumerate_leaves (b200tsdf* h, int nlevels, bool occupied, const char* what, void** out, size_t* n)
+// order.  The records land in `out` (3 x 32 bits each, malloc'ed, owned by the handle).  The brick list lives in the handle's
+// grow-only scratch (pool-sized, like the query buffers); the record and sort buffers are sized by the result (hundreds of MB
+// for a large volume) and are released before returning rather than kept on the handle.
+int enumerate_leaves (b200tsdf* h, int nlevels, bool occupied, const char* what, void*& out, size_t* n)
 {
   if (!h->has_volume) return h->fail (B200TSDF_ESTATE, std::string (what) + " before reset()");
   if (h->p.shard_count > 1)
@@ -1633,72 +1682,35 @@ int enumerate_leaves (b200tsdf* h, int nlevels, bool occupied, const char* what,
                     "enumerate on the replica built by b200tsdf_gather_volume");
   cudaSetDevice (h->device);
   if (int rc = pending_device_err (h)) return rc;
-  std::free (*out); *out = nullptr; *n = 0;
   const Params& p = h->p;
   cudaStream_t s = h->stream;
-  uint32_t *d_rec = nullptr, *d_rec2 = nullptr; unsigned long long* d_k = nullptr;
-  auto release = [&] () { cudaStreamSynchronize (s); cudaFree (d_rec); cudaFree (d_rec2); cudaFree (d_k); };
-  auto nomem = [&] (const char* m) { release (); cudaGetLastError (); return h->fail (B200TSDF_ENOMEM, m); };
-  // CK that frees this call's device buffers on the way out
-#define LCK(call)                                                                                  \
-  do {                                                                                             \
-    cudaError_t e_ = (call);                                                                       \
-    if (e_ != cudaSuccess) { release (); return h->fail (B200TSDF_ECUDA, std::string (#call) + ": " + cudaGetErrorString (e_)); } \
-  } while (0)
   unsigned long long count = 0;
-  uint32_t* d_sorted = nullptr;
   if (!occupied && nlevels >= 0 && (nlevels < p.C || nlevels == 0))
   {
     // every node of that depth exists (Octree::init) and none is ever pruned: 8^nlevels records, already in order
     count = 1ull << (3 * nlevels);
-    if (cudaMalloc (&d_rec, count * 12) != cudaSuccess) return nomem ("device allocation failed (voxel centres)");
-    k_leaves_level<<<(unsigned) ((count + 127) / 128), 128, 0, s>>> (p, nlevels, count, d_rec);
-    d_sorted = d_rec;
+    DevBuf<uint32_t> rec (s);
+    if (rec.alloc (count * 3)) return alloc_failed (h, "voxel centres");
+    k_leaves_level<<<(unsigned) ((count + 127) / 128), 128, 0, s>>> (p, nlevels, count, rec);
+    if (int rc = download (h, rec, count * 12, out)) return rc;
   }
   else
   {
-    int* d_nb = h->d_count + 40;
-    unsigned long long* d_total = h->d_stats + ST_SCRATCH;
-    if (int rc = h->scratch (h->pool * sizeof (int))) return rc;
-    int* d_list = (int*) h->d_scratch;
-    LCK (cudaMemsetAsync (d_nb, 0, sizeof (int), s));
-    LCK (cudaMemsetAsync (d_total, 0, sizeof (unsigned long long), s));
-    k_list_bricks<<<(unsigned) ((h->pool + 255) / 256), 256, 0, s>>> (p, d_list, d_nb);
-    int nb = 0;
-    LCK (cudaMemcpyAsync (&nb, d_nb, sizeof (int), cudaMemcpyDeviceToHost, s));
-    LCK (cudaStreamSynchronize (s));
-    const int root_n = (int) h->root_n, occ = occupied ? 1 : 0;
-    const unsigned bgrid = (unsigned) (((size_t) nb * 32 + 127) / 128), rgrid = (unsigned) ((root_n + 127) / 128);
-    if (nb) k_leaves_bricks<false><<<bgrid, 128, 0, s>>> (p, d_list, nb, nlevels, occ, d_total, nullptr, nullptr);
-    k_leaves_roots<false><<<rgrid, 128, 0, s>>> (p, nlevels, occ, d_total, nullptr, nullptr);
-    LCK (cudaMemcpyAsync (&count, d_total, sizeof (count), cudaMemcpyDeviceToHost, s));
-    LCK (cudaStreamSynchronize (s));
-    if (count)
+    int* list = nullptr;
+    const int nb = list_bricks (h, list);
+    if (nb < 0) return nb;
+    const int occ = occupied ? 1 : 0;
+    const unsigned bgrid = (unsigned) (((size_t) nb * 32 + 127) / 128), rgrid = (unsigned) ((h->root_n + 127) / 128);
+    auto launch = [&] (auto emit, unsigned long long* total, unsigned long long* keys, void* rec, unsigned char*)
     {
-      if (cudaMalloc (&d_rec, count * 12) != cudaSuccess || cudaMalloc (&d_rec2, count * 12) != cudaSuccess
-          || cudaMalloc (&d_k, count * sizeof (unsigned long long)) != cudaSuccess)
-        return nomem ("device allocation failed (leaf records)");
-      LCK (cudaMemsetAsync (d_total, 0, sizeof (unsigned long long), s));
-      if (nb) k_leaves_bricks<true><<<bgrid, 128, 0, s>>> (p, d_list, nb, nlevels, occ, d_total, d_k, d_rec);
-      k_leaves_roots<true><<<rgrid, 128, 0, s>>> (p, nlevels, occ, d_total, d_k, d_rec);
-      // emission order depends on the hash layout and on atomics: sort into depth-first order
-      const int e = b2_sort_records (s, (size_t) count, 3 * p.L, d_k, 3, d_rec, nullptr, d_rec2, nullptr);
-      if (e == (int) cudaErrorMemoryAllocation) return nomem ("device allocation failed (leaf sort)");
-      if (e) { release (); return h->fail (B200TSDF_ECUDA, std::string ("leaf sort: ") + cudaGetErrorString ((cudaError_t) e)); }
-      d_sorted = d_rec2;
-    }
+      constexpr bool E = decltype (emit)::value;
+      if (nb) k_leaves_bricks<E><<<bgrid, 128, 0, s>>> (p, list, nb, nlevels, occ, total, keys, (uint32_t*) rec);
+      k_leaves_roots<E><<<rgrid, 128, 0, s>>> (p, nlevels, occ, total, keys, (uint32_t*) rec);
+    };
+    if (int rc = sorted_records (h, "leaf records", 3, 3 * p.L, launch, out, nullptr, count)) return rc;
   }
-#undef LCK
-  void* host = std::malloc (std::max<size_t> ((size_t) count, 1) * 12);
-  if (!host) return nomem ("host allocation failed (leaf records)");
-  cudaError_t e = cudaSuccess;
-  if (count) e = cudaMemcpyAsync (host, d_sorted, count * 12, cudaMemcpyDeviceToHost, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize (s);
-  if (e == cudaSuccess) e = cudaGetLastError ();
-  release ();
-  if (e != cudaSuccess) { std::free (host); return h->fail (B200TSDF_ECUDA, std::string (what) + ": " + cudaGetErrorString (e)); }
   h->d2h_bytes += (long long) (count * 12);
-  *out = host; *n = (size_t) count;
+  *n = (size_t) count;
   return check_device_err (h);
 }
 
@@ -1710,11 +1722,9 @@ int b200tsdf_voxel_centers (b200tsdf_t* h, int nlevels, float** xyz, size_t* n)
 {
   if (!h || !xyz || !n) return B200TSDF_EINVAL;
   *xyz = nullptr; *n = 0;
-  void* buf = h->leaf_xyz;
-  int rc = enumerate_leaves (h, nlevels, false, "getVoxelCenters", &buf, n);
-  h->leaf_xyz = (float*) buf;
+  int rc = enumerate_leaves (h, nlevels, false, "getVoxelCenters", h->leaf_xyz, n);
   if (rc) { *n = 0; return rc; }
-  *xyz = h->leaf_xyz;
+  *xyz = (float*) h->leaf_xyz;
   return B200TSDF_OK;
 }
 
@@ -1722,11 +1732,9 @@ int b200tsdf_occupied_voxel_indices (b200tsdf_t* h, int32_t** ijk, size_t* n)
 {
   if (!h || !ijk || !n) return B200TSDF_EINVAL;
   *ijk = nullptr; *n = 0;
-  void* buf = h->leaf_ijk;
-  int rc = enumerate_leaves (h, -1, true, "getOccupiedVoxelIndices", &buf, n);
-  h->leaf_ijk = (int32_t*) buf;
+  int rc = enumerate_leaves (h, -1, true, "getOccupiedVoxelIndices", h->leaf_ijk, n);
   if (rc) { *n = 0; return rc; }
-  *ijk = h->leaf_ijk;
+  *ijk = (int32_t*) h->leaf_ijk;
   return B200TSDF_OK;
 }
 
@@ -1832,50 +1840,40 @@ int take_snapshot (b200tsdf* h, Snapshot& S)
   if (rc) return rc;
   const Params& dp = h->p;
   cudaStream_t s = h->stream;
-  int* d_list = nullptr; int* d_n = h->d_count + 40;
-  CK (cudaMalloc (&d_list, h->pool * sizeof (int)));
-  CK (cudaMemsetAsync (d_n, 0, sizeof (int), s));
-  k_list_bricks<<<(unsigned) ((h->pool + 255) / 256), 256, 0, s>>> (dp, d_list, d_n);
-  int nb = 0;
-  CK (cudaMemcpyAsync (&nb, d_n, sizeof (int), cudaMemcpyDeviceToHost, s));
-  CK (cudaStreamSynchronize (s));
+  int* d_list = nullptr;
+  const int nb = list_bricks (h, d_list);
+  if (nb < 0) return nb;
   std::vector<int> list (nb);
   std::vector<uint64_t> dkeys (h->pool);
   CK (cudaMemcpy (dkeys.data (), dp.keys, h->pool * sizeof (uint64_t), cudaMemcpyDeviceToHost));
   if (nb) CK (cudaMemcpy (list.data (), d_list, (size_t) nb * sizeof (int), cudaMemcpyDeviceToHost));
-  float2* g_nodes = nullptr; uint32_t* g_split = nullptr; uchar4* g_rgb = nullptr; float* g_M = nullptr; int* g_ns = nullptr;
-  size_t nbz = std::max (nb, 1);
-  CK (cudaMalloc (&g_nodes, nbz * BRICK_NODES * sizeof (float2)));
-  CK (cudaMalloc (&g_split, nbz * BRICK_SPLIT_WORDS * sizeof (uint32_t)));
-  if (dp.rgb) CK (cudaMalloc (&g_rgb, nbz * BRICK_NODES * sizeof (uchar4)));
-  if (dp.M) { CK (cudaMalloc (&g_M, nbz * BRICK_NODES * sizeof (float))); CK (cudaMalloc (&g_ns, nbz * BRICK_NODES * sizeof (int))); }
-  if (nb) k_gather_bricks<<<nb, 128, 0, s>>> (dp, d_list, nb, g_nodes, g_split, g_rgb, g_M, g_ns);
+  const size_t nn = (size_t) nb * BRICK_NODES;
+  DevBuf<float2> g_nodes (s); DevBuf<uint32_t> g_split (s); DevBuf<uchar4> g_rgb (s); DevBuf<float> g_M (s); DevBuf<int> g_ns (s); DevBuf<float4> g_q (s);
+  CK (g_nodes.alloc (nn)); CK (g_split.alloc ((size_t) nb * BRICK_SPLIT_WORDS));
+  if (dp.rgb) CK (g_rgb.alloc (nn));
+  if (dp.M) { CK (g_M.alloc (nn)); CK (g_ns.alloc (nn)); }
+  if (dp.rgbn) CK (g_q.alloc (nn));
+  if (nb)
+  {
+    k_gather_bricks<<<nb, 128, 0, s>>> (dp, d_list, nb, g_nodes, g_split, g_rgb, g_M, g_ns);
+    if (dp.rgbn) k_gather_rgbn<<<nb, 128, 0, s>>> (dp, d_list, nb, g_q);
+  }
   CK (cudaStreamSynchronize (s));
-  std::vector<float2> c_nodes ((size_t) nb * BRICK_NODES); std::vector<uint32_t> c_split ((size_t) nb * BRICK_SPLIT_WORDS);
-  std::vector<uchar4> c_rgb; std::vector<float> c_M; std::vector<int> c_ns;
+  std::vector<float2> c_nodes (nn); std::vector<uint32_t> c_split ((size_t) nb * BRICK_SPLIT_WORDS);
+  std::vector<uchar4> c_rgb; std::vector<float> c_M; std::vector<int> c_ns; std::vector<float4> c_rgbn;
   if (nb)
   {
     CK (cudaMemcpy (c_nodes.data (), g_nodes, c_nodes.size () * sizeof (float2), cudaMemcpyDeviceToHost));
     CK (cudaMemcpy (c_split.data (), g_split, c_split.size () * sizeof (uint32_t), cudaMemcpyDeviceToHost));
-    if (dp.rgb) { c_rgb.resize ((size_t) nb * BRICK_NODES); CK (cudaMemcpy (c_rgb.data (), g_rgb, c_rgb.size () * sizeof (uchar4), cudaMemcpyDeviceToHost)); }
+    if (dp.rgb) { c_rgb.resize (nn); CK (cudaMemcpy (c_rgb.data (), g_rgb, nn * sizeof (uchar4), cudaMemcpyDeviceToHost)); }
     if (dp.M)
     {
-      c_M.resize ((size_t) nb * BRICK_NODES); c_ns.resize ((size_t) nb * BRICK_NODES);
-      CK (cudaMemcpy (c_M.data (), g_M, c_M.size () * sizeof (float), cudaMemcpyDeviceToHost));
-      CK (cudaMemcpy (c_ns.data (), g_ns, c_ns.size () * sizeof (int), cudaMemcpyDeviceToHost));
+      c_M.resize (nn); c_ns.resize (nn);
+      CK (cudaMemcpy (c_M.data (), g_M, nn * sizeof (float), cudaMemcpyDeviceToHost));
+      CK (cudaMemcpy (c_ns.data (), g_ns, nn * sizeof (int), cudaMemcpyDeviceToHost));
     }
+    if (dp.rgbn) { c_rgbn.resize (nn); CK (cudaMemcpy (c_rgbn.data (), g_q, nn * sizeof (float4), cudaMemcpyDeviceToHost)); }
   }
-  std::vector<float4> c_rgbn;
-  if (dp.rgbn)
-  {
-    float4* g_q = nullptr;
-    CK (cudaMalloc (&g_q, nbz * BRICK_NODES * sizeof (float4)));
-    if (nb) k_gather_rgbn<<<nb, 128, 0, s>>> (dp, d_list, nb, g_q);
-    c_rgbn.resize ((size_t) nb * BRICK_NODES);
-    if (nb) CK (cudaMemcpy (c_rgbn.data (), g_q, c_rgbn.size () * sizeof (float4), cudaMemcpyDeviceToHost));
-    cudaFree (g_q);
-  }
-  cudaFree (d_list); cudaFree (g_nodes); cudaFree (g_split); cudaFree (g_rgb); cudaFree (g_M); cudaFree (g_ns);
   // compact directory
   size_t hp = 16;
   while (hp < (size_t) nb * 2) hp <<= 1;
@@ -1893,9 +1891,9 @@ int take_snapshot (b200tsdf* h, Snapshot& S)
   S.p.err = &S.err;
   for (int i = 0; i < nb; ++i)
   {
-    uint64_t key = dkeys[list[i]];
-    int t = (int) (key >> 60) - 1;
-    int slot = find_or_insert_brick (S.p, t, (int) ((key >> 40) & 0xFFFFF), (int) ((key >> 20) & 0xFFFFF), (int) (key & 0xFFFFF));
+    int t, bx, by, bz;
+    brick_key_decode (dkeys[list[i]], t, bx, by, bz);
+    int slot = find_or_insert_brick (S.p, t, bx, by, bz);
     std::memcpy (&S.nodes[(size_t) slot * BRICK_NODES], &c_nodes[(size_t) i * BRICK_NODES], BRICK_NODES * sizeof (float2));
     std::memcpy (&S.split[(size_t) slot * BRICK_SPLIT_WORDS], &c_split[(size_t) i * BRICK_SPLIT_WORDS], BRICK_SPLIT_WORDS * sizeof (uint32_t));
     if (dp.rgb) std::memcpy (&S.rgb[(size_t) slot * BRICK_NODES], &c_rgb[(size_t) i * BRICK_NODES], BRICK_NODES * sizeof (uchar4));
@@ -2205,21 +2203,13 @@ int b200tsdf_load (b200tsdf_t* h, const char* path)
   int nb = (int) L.keys.size ();
   if (nb)
   {
-    uint64_t* dk = nullptr; float2* dn = nullptr; uint32_t* ds = nullptr; uchar4* dc = nullptr; float* dM = nullptr; int* dns = nullptr;
-    CK (cudaMalloc (&dk, (size_t) nb * 8)); CK (cudaMalloc (&dn, (size_t) nb * BRICK_NODES * sizeof (float2))); CK (cudaMalloc (&ds, (size_t) nb * BRICK_SPLIT_WORDS * 4));
-    CK (cudaMemcpy (dk, L.keys.data (), (size_t) nb * 8, cudaMemcpyHostToDevice));
-    CK (cudaMemcpy (dn, L.nodes.data (), (size_t) nb * BRICK_NODES * sizeof (float2), cudaMemcpyHostToDevice));
-    CK (cudaMemcpy (ds, L.split.data (), (size_t) nb * BRICK_SPLIT_WORDS * 4, cudaMemcpyHostToDevice));
-    if (p.rgb) { CK (cudaMalloc (&dc, (size_t) nb * BRICK_NODES * 4)); CK (cudaMemcpy (dc, L.rgbv.data (), (size_t) nb * BRICK_NODES * 4, cudaMemcpyHostToDevice)); }
-    if (p.M)
-    {
-      CK (cudaMalloc (&dM, (size_t) nb * BRICK_NODES * 4)); CK (cudaMalloc (&dns, (size_t) nb * BRICK_NODES * 4));
-      CK (cudaMemcpy (dM, L.Mv.data (), (size_t) nb * BRICK_NODES * 4, cudaMemcpyHostToDevice));
-      CK (cudaMemcpy (dns, L.nsv.data (), (size_t) nb * BRICK_NODES * 4, cudaMemcpyHostToDevice));
-    }
-    k_load_bricks<<<nb, 128, 0, h->stream>>> (p, dk, nb, dn, ds, dc, dM, dns);
-    CK (cudaStreamSynchronize (h->stream));
-    cudaFree (dk); cudaFree (dn); cudaFree (ds); cudaFree (dc); cudaFree (dM); cudaFree (dns);
+    cudaStream_t s = h->stream;
+    DevBuf<uint64_t> dk (s); DevBuf<float2> dn (s); DevBuf<uint32_t> ds (s); DevBuf<uchar4> dc (s); DevBuf<float> dM (s); DevBuf<int> dns (s);
+    CK (dk.upload (L.keys)); CK (dn.upload (L.nodes)); CK (ds.upload (L.split));
+    if (p.rgb) CK (dc.upload (L.rgbv));
+    if (p.M) { CK (dM.upload (L.Mv)); CK (dns.upload (L.nsv)); }
+    k_load_bricks<<<nb, 128, 0, s>>> (p, dk, nb, dn, ds, dc, dM, dns);
+    CK (cudaStreamSynchronize (s));
   }
   h->is_empty = is_empty != 0;
   return check_device_err (h);
@@ -2252,9 +2242,9 @@ int b200tsdf_export_shard (b200tsdf_t* h, void* buf, size_t capacity, size_t* nb
   {
     uint64_t key = p.keys[s];
     if (key == KEY_EMPTY) continue;
-    int t = (int) (key >> 60) - 1;
+    int t, bx, by, bz;
+    brick_key_decode (key, t, bx, by, bz);
     int sh = tier_root_level (p, t) - p.C;
-    int bx = (int) ((key >> 40) & 0xFFFFF), by = (int) ((key >> 20) & 0xFFFFF), bz = (int) (key & 0xFFFFF);
     if (owns_cell (p, bx >> sh, by >> sh, bz >> sh)) bricks.push_back (s);
   }
   const size_t root_rec = 4 + 8 + 1 + 4 + 4 + 4, brick_rec = 8 + BRICK_NODES * 8 + BRICK_SPLIT_WORDS * 4 + (color ? BRICK_NODES * 4 : 0) + (var ? BRICK_NODES * 8 : 0);
@@ -2321,25 +2311,20 @@ int b200tsdf_import_shard (b200tsdf_t* h, const void* buf, size_t nbytes)
     if (var) { std::memcpy (&Mv[i * BRICK_NODES], o, BRICK_NODES * 4); o += BRICK_NODES * 4; std::memcpy (&nsv[i * BRICK_NODES], o, BRICK_NODES * 4); o += BRICK_NODES * 4; }
   }
   cudaStream_t s = h->stream;
-  auto up = [&] (const void* src, size_t bytes, void** dst) -> cudaError_t { if (!bytes) { *dst = nullptr; return cudaSuccess; } cudaError_t e = cudaMalloc (dst, bytes); if (e != cudaSuccess) return e; return cudaMemcpy (*dst, src, bytes, cudaMemcpyHostToDevice); };
-  void *d_idx = nullptr, *d_dw = nullptr, *d_sp = nullptr, *d_rgb = nullptr, *d_M = nullptr, *d_ns = nullptr;
   if (nr)
   {
-    CK (up (ridx.data (), nr * 4, &d_idx)); CK (up (rdw.data (), nr * 8, &d_dw)); CK (up (rsp.data (), nr, &d_sp));
-    CK (up (rrgb.data (), nr * 4, &d_rgb)); CK (up (rM.data (), nr * 4, &d_M)); CK (up (rns.data (), nr * 4, &d_ns));
-    k_import_roots<<<(unsigned) ((nr + 127) / 128), 128, 0, s>>> (p, (int) nr, (const int*) d_idx, (const float2*) d_dw, (const unsigned char*) d_sp, (const uchar4*) d_rgb, (const float*) d_M, (const int*) d_ns);
+    DevBuf<int> d_idx (s); DevBuf<float2> d_dw (s); DevBuf<unsigned char> d_sp (s); DevBuf<uchar4> d_rgb (s); DevBuf<float> d_M (s); DevBuf<int> d_ns (s);
+    CK (d_idx.upload (ridx)); CK (d_dw.upload (rdw)); CK (d_sp.upload (rsp)); CK (d_rgb.upload (rrgb)); CK (d_M.upload (rM)); CK (d_ns.upload (rns));
+    k_import_roots<<<(unsigned) ((nr + 127) / 128), 128, 0, s>>> (p, (int) nr, d_idx, d_dw, d_sp, d_rgb, d_M, d_ns);
     CK (cudaStreamSynchronize (s));
-    cudaFree (d_idx); cudaFree (d_dw); cudaFree (d_sp); cudaFree (d_rgb); cudaFree (d_M); cudaFree (d_ns);
   }
   if (nb)
   {
-    void *dk = nullptr, *dn = nullptr, *ds = nullptr, *dc = nullptr, *dM = nullptr, *dns = nullptr;
-    CK (up (keys.data (), nb * 8, &dk)); CK (up (nodes.data (), nb * BRICK_NODES * 8, &dn)); CK (up (split.data (), nb * BRICK_SPLIT_WORDS * 4, &ds));
-    if (color) CK (up (rgb.data (), nb * BRICK_NODES * 4, &dc));
-    if (var) { CK (up (Mv.data (), nb * BRICK_NODES * 4, &dM)); CK (up (nsv.data (), nb * BRICK_NODES * 4, &dns)); }
-    k_load_bricks<<<(unsigned) nb, 128, 0, s>>> (p, (const uint64_t*) dk, (int) nb, (const float2*) dn, (const uint32_t*) ds, (const uchar4*) dc, (const float*) dM, (const int*) dns);
+    DevBuf<uint64_t> dk (s); DevBuf<float2> dn (s); DevBuf<uint32_t> ds (s); DevBuf<uchar4> dc (s); DevBuf<float> dM (s); DevBuf<int> dns (s);
+    CK (dk.upload (keys)); CK (dn.upload (nodes)); CK (ds.upload (split));
+    CK (dc.upload (rgb)); CK (dM.upload (Mv)); CK (dns.upload (nsv));      // (empty without colour / variance: null)
+    k_load_bricks<<<(unsigned) nb, 128, 0, s>>> (p, dk, (int) nb, dn, ds, dc, dM, dns);
     CK (cudaStreamSynchronize (s));
-    cudaFree (dk); cudaFree (dn); cudaFree (ds); cudaFree (dc); cudaFree (dM); cudaFree (dns);
   }
   h->is_empty = false;
   return check_device_err (h);

@@ -338,25 +338,20 @@ int b200tsdf_gather_volume (b200tsdf_t* h, b200tsdf_t* full, int root)
   const bool color = p.rgb != nullptr;
   const size_t rn = h->root_n, rsw = (rn + 31) / 32;
   // what this rank owns, packed on the device
-  int* d_list = nullptr; int* d_n = h->d_count + 40;
-  long long* d_counts = nullptr;
-  CK (cudaMalloc (&d_list, h->pool * sizeof (int)));
-  CK (cudaMalloc (&d_counts, (size_t) (nr + 1) * sizeof (long long)));
-  CK (cudaMemsetAsync (d_n, 0, sizeof (int), s));
-  k_list_bricks<<<(unsigned) ((h->pool + 255) / 256), 256, 0, s>>> (p, d_list, d_n);
-  int nb = 0;
-  CK (cudaMemcpyAsync (&nb, d_n, sizeof (int), cudaMemcpyDeviceToHost, s));
-  CK (cudaStreamSynchronize (s));
+  int* d_list = nullptr;
+  const int nb = list_bricks (h, d_list);
+  if (nb < 0) return nb;
+  DevBuf<long long> d_counts (s);
+  CK (d_counts.alloc ((size_t) nr + 1));
   long long mine = nb;
   CK (cudaMemcpyAsync (d_counts + nr, &mine, sizeof (long long), cudaMemcpyHostToDevice, s));
   NK (a.AllGather (d_counts + nr, d_counts, 1, ncclInt64, (ncclComm_t) h->comm, s));
   std::vector<long long> counts (nr);
   CK (cudaMemcpyAsync (counts.data (), d_counts, (size_t) nr * sizeof (long long), cudaMemcpyDeviceToHost, s));
   CK (cudaStreamSynchronize (s));
-  const size_t nbz = (size_t) std::max (nb, 1);
-  uint64_t* g_keys = nullptr; float2* g_nodes = nullptr; uint32_t* g_split = nullptr; uchar4* g_rgb = nullptr;
-  CK (cudaMalloc (&g_keys, nbz * 8)); CK (cudaMalloc (&g_nodes, nbz * BRICK_NODES * sizeof (float2))); CK (cudaMalloc (&g_split, nbz * BRICK_SPLIT_WORDS * 4));
-  if (color) CK (cudaMalloc (&g_rgb, nbz * BRICK_NODES * 4));
+  DevBuf<uint64_t> g_keys (s); DevBuf<float2> g_nodes (s); DevBuf<uint32_t> g_split (s); DevBuf<uchar4> g_rgb (s);
+  CK (g_keys.alloc (nb)); CK (g_nodes.alloc ((size_t) nb * BRICK_NODES)); CK (g_split.alloc ((size_t) nb * BRICK_SPLIT_WORDS));
+  if (color) CK (g_rgb.alloc ((size_t) nb * BRICK_NODES));
   if (nb)
   {
     k_gather_keys<<<(nb + 255) / 256, 256, 0, s>>> (p, d_list, nb, g_keys);
@@ -388,11 +383,11 @@ int b200tsdf_gather_volume (b200tsdf_t* h, b200tsdf_t* full, int root)
     if (nb) k_load_bricks<<<nb, 128, 0, s>>> (fp, g_keys, nb, g_nodes, g_split, g_rgb, nullptr, nullptr);
     long long maxb = 1;
     for (int r = 0; r < nr; ++r) if (r != root) maxb = std::max (maxb, counts[r]);
-    float2* r_dw = nullptr; uint32_t* r_split = nullptr; uchar4* r_rgb = nullptr;
-    uint64_t* b_keys = nullptr; float2* b_nodes = nullptr; uint32_t* b_split = nullptr; uchar4* b_rgb = nullptr;
-    CK (cudaMalloc (&r_dw, rn * 8)); CK (cudaMalloc (&r_split, rsw * 4)); if (color) CK (cudaMalloc (&r_rgb, rn * 4));
-    CK (cudaMalloc (&b_keys, (size_t) maxb * 8)); CK (cudaMalloc (&b_nodes, (size_t) maxb * BRICK_NODES * 8)); CK (cudaMalloc (&b_split, (size_t) maxb * BRICK_SPLIT_WORDS * 4));
-    if (color) CK (cudaMalloc (&b_rgb, (size_t) maxb * BRICK_NODES * 4));
+    DevBuf<float2> r_dw (s); DevBuf<uint32_t> r_split (s); DevBuf<uchar4> r_rgb (s);
+    DevBuf<uint64_t> b_keys (s); DevBuf<float2> b_nodes (s); DevBuf<uint32_t> b_split (s); DevBuf<uchar4> b_rgb (s);
+    CK (r_dw.alloc (rn)); CK (r_split.alloc (rsw)); if (color) CK (r_rgb.alloc (rn));
+    CK (b_keys.alloc ((size_t) maxb)); CK (b_nodes.alloc ((size_t) maxb * BRICK_NODES)); CK (b_split.alloc ((size_t) maxb * BRICK_SPLIT_WORDS));
+    if (color) CK (b_rgb.alloc ((size_t) maxb * BRICK_NODES));
     for (int r = 0; r < nr && rc_out == B200TSDF_OK; ++r)
     {
       if (r == root) continue;
@@ -413,14 +408,12 @@ int b200tsdf_gather_volume (b200tsdf_t* h, b200tsdf_t* full, int root)
       if (cb) k_load_bricks<<<(unsigned) cb, 128, 0, s>>> (fp, b_keys, (int) cb, b_nodes, b_split, b_rgb, nullptr, nullptr);
       CK (cudaStreamSynchronize (s));                       // the receive buffers are reused for the next rank
     }
-    cudaFree (r_dw); cudaFree (r_split); cudaFree (r_rgb); cudaFree (b_keys); cudaFree (b_nodes); cudaFree (b_split); cudaFree (b_rgb);
     full->is_empty = false;
     // errors raised by the scatter (pool of the full handle too small) are on the FULL handle's flag
     int e = 0;
     cudaMemcpy (&e, full->d_err, sizeof (int), cudaMemcpyDeviceToHost);
     if (e & ERR_POOL_FULL) rc_out = h->fail (B200TSDF_ENOMEM, "brick pool of the full handle exhausted (raise its pool_log2)");
   }
-  cudaFree (d_list); cudaFree (d_counts); cudaFree (g_keys); cudaFree (g_nodes); cudaFree (g_split); cudaFree (g_rgb);
   return rc_out;
 }
 

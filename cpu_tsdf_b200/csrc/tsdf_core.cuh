@@ -251,6 +251,8 @@ B2_HD int split_word_base (int k) { return k == 1 ? 0 : (k == 2 ? 1 : 4); }
 
 B2_HD uint64_t brick_key (int t, int bx, int by, int bz)
 { return ((uint64_t) (t + 1) << 60) | ((uint64_t) bx << 40) | ((uint64_t) by << 20) | (uint64_t) bz; }
+B2_HD void brick_key_decode (uint64_t key, int& t, int& bx, int& by, int& bz)
+{ t = (int) (key >> 60) - 1; bx = (int) ((key >> 40) & 0xFFFFF); by = (int) ((key >> 20) & 0xFFFFF); bz = (int) (key & 0xFFFFF); }
 B2_HD uint32_t hash_key (uint64_t k)
 {
   k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
@@ -1190,6 +1192,16 @@ B2_HD bool leaf_selected (int level, bool exists, bool has_children, int nlevels
   return !occupied || (w > 0.f && fabsf (d) < 1.f);
 }
 
+// whether the root of brick (t, bx, by, bz) has children, i.e. whether the brick's nodes exist at all
+B2_HD bool brick_root_is_split (const Params& p, int t, int bx, int by, int bz)
+{
+  const int R = tier_root_level (p, t);
+  if (R < p.C) return true;
+  NodePos r;
+  if (!locate_node (p, R, bx, by, bz, r)) return false;
+  return is_split (p, r);
+}
+
 // node i (0..583) of the brick rooted at level R, coordinates (bx, by, bz): its level and coordinates, whether it exists
 // and whether it has children.  sw = the brick's split words, root_split = whether the brick's root has children.
 // Levels above the coarse depth always have children (Octree::init), whatever their storage says.
@@ -1207,6 +1219,15 @@ B2_HD BrickNode brick_node (const Params& p, const uint32_t* sw, int R, int bx, 
   for (int q = k - 1; q >= 0; --q) { int c = (j >> (3 * q)) & 7; lx = (lx << 1) | (c >> 2); ly = (ly << 1) | ((c >> 1) & 1); lz = (lz << 1) | (c & 1); }
   b.x = (bx << k) | lx; b.y = (by << k) | ly; b.z = (bz << k) | lz;
   return b;
+}
+// the NodePos of node i of the brick in `slot` (slot -1: the root-array entry i)
+B2_HD NodePos brick_node_pos (const Params& p, const BrickNode& b, int slot, int i)
+{
+  NodePos n;
+  n.level = b.level; n.x = b.x; n.y = b.y; n.z = b.z;
+  n.cx = center1d (p, b.level, b.x); n.cy = center1d (p, b.level, b.y); n.cz = center1d (p, b.level, b.z);
+  n.size = level_size (p, b.level); n.slot = slot; n.idx = i;
+  return n;
 }
 
 B2_HD uint32_t float_bits (float f)

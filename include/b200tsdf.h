@@ -157,7 +157,7 @@ int  b200tsdf_render (b200tsdf_t* h, const double* pose_c2w, int downsample, voi
  * 108-143): triangle soup, 3 vertices per triangle, global transform applied.
  * color_mode 0 none / 1 setColorByRGB / 2 setColorByConfidence.  *verts (3 floats per vertex)
  * and *rgb (3 bytes per vertex, or NULL) are library-owned until the next mesh call or
- * b200tsdf_free. */
+ * b200tsdf_free.  B200TSDF_ENOMEM when the triangle or sort buffers do not fit. */
 int  b200tsdf_mesh (b200tsdf_t* h, float w_min, int color_mode, float** verts, uint8_t** rgb, size_t* nverts);
 void b200tsdf_free (void* p);
 

@@ -65,6 +65,31 @@ static void collect (const Params& p, const NodePos& n, std::vector<Rec>& out)
   for (int c = 0; c < 8; ++c) collect (p, make_child (p, n, c, cs), out);
 }
 
+// The kernels' walk of the flat layout (k_mesh_bricks / k_leaves_bricks, then k_mesh_roots / k_leaves_roots) in plain loops:
+// every node of every claimed brick whose root has children, then every root-array entry.  visit (b, dw, slot, i) gets the
+// node as brick_node describes it, its {sdf, weight} and its storage (slot -1: root array, i = root index).
+template <typename Visit>
+static void walk_nodes (const Params& p, const Visit& visit)
+{
+  for (size_t slot = 0; slot <= p.pool_mask; ++slot)
+  {
+    if (p.keys[slot] == KEY_EMPTY) continue;
+    int t, bx, by, bz;
+    brick_key_decode (p.keys[slot], t, bx, by, bz);
+    if (!brick_root_is_split (p, t, bx, by, bz)) continue;
+    const uint32_t* sw = p.split + slot * BRICK_SPLIT_WORDS;
+    for (int i = 0; i < BRICK_NODES; ++i)
+      visit (brick_node (p, sw, tier_root_level (p, t), bx, by, bz, true, i), p.nodes[slot * BRICK_NODES + i], (int) slot, i);
+  }
+  const int n = 1 << p.Rtop;
+  for (int i = 0; i < n * n * n; ++i)
+  {
+    const NodePos nd = make_root (p, i / (n * n), (i / n) % n, i % n);
+    BrickNode b; b.level = p.Rtop; b.x = nd.x; b.y = nd.y; b.z = nd.z; b.exists = true; b.split = is_split (p, nd);
+    visit (b, p.root_dw[nd.idx], -1, nd.idx);
+  }
+}
+
 extern "C" {
 
 Emu* emu_create (const b200tsdf_config* cfg) { Emu* e = new Emu; e->cfg = *cfg; return e; }
@@ -210,33 +235,18 @@ long long emu_mesh (Emu* e, float w_min, int color_mode, const float** verts, co
   const Params& p = e->p;
   McParams mc;
   make_mc_params (e->cfg, p, w_min, color_mode, mc);
-  std::vector<Rec> recs;
   e->mesh_v.clear (); e->mesh_c.clear ();
-  // every leaf, any level, visited in an arbitrary (stack) order and then sorted by the order key
+  // k_mesh_bricks / k_mesh_roots: one cube per existing leaf at or below the coarse depth, then sorted by the order key
   std::vector<std::pair<unsigned long long, size_t> > order;
-  int n = 1 << p.C;
-  std::vector<NodePos> stack;
-  for (int x = 0; x < n; ++x) for (int y = 0; y < n; ++y) for (int z = 0; z < n; ++z)
+  walk_nodes (p, [&] (const BrickNode& b, float2 dw, int slot, int i)
   {
-    NodePos nd;
-    if (!locate_node (p, p.C, x, y, z, nd)) return -1;
-    stack.push_back (nd);
-    while (!stack.empty ())
-    {
-      NodePos q = stack.back (); stack.pop_back ();
-      if (is_split (p, q))
-      {
-        int cs = children_slot (p, q, false);
-        for (int c = 0; c < 8 && cs >= 0; ++c) stack.push_back (make_child (p, q, c, cs));
-        continue;
-      }
-      float2 dw = *node_dw (p, q);
-      float v[45]; unsigned char cc[45];
-      int nt = mc_leaf (p, mc, q, dw.x, dw.y, mc_tables::edge_table, mc_tables::tri_table, v, color_mode ? cc : nullptr);
-      for (int i = 0; i < 9 * nt; ++i) { e->mesh_v.push_back (v[i]); if (color_mode) e->mesh_c.push_back (cc[i]); }
-      for (int t = 0; t < nt; ++t) order.push_back ({ (mc_order_key (p, q) << 3) | (unsigned long long) t, order.size () });
-    }
-  }
+    if (!b.exists || b.split || b.level < p.C) return;
+    const NodePos q = brick_node_pos (p, b, slot, i);
+    float v[45]; unsigned char cc[45];
+    int nt = mc_leaf (p, mc, q, dw.x, dw.y, mc_tables::edge_table, mc_tables::tri_table, v, color_mode ? cc : nullptr);
+    for (int k = 0; k < 9 * nt; ++k) { e->mesh_v.push_back (v[k]); if (color_mode) e->mesh_c.push_back (cc[k]); }
+    for (int t = 0; t < nt; ++t) order.push_back ({ (mc_order_key (p, q) << 3) | (unsigned long long) t, order.size () });
+  });
   // the engine sorts its (unordered) emission by mc_order_key: the result must be the reference's own order
   std::sort (order.begin (), order.end ());
   {

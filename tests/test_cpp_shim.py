@@ -7,19 +7,19 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "cpp", "shim_example.cpp")
-EXE = os.path.join(ROOT, "tests", "cpp", "shim_example")
 CXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
 
 
-def build(engine_lib):
+def build(engine_lib, out_dir):
     libdir = os.path.dirname(engine_lib)
-    subprocess.run([CXX, "-std=c++17", "-O1", SRC, "-o", EXE, f"-L{libdir}", "-lb200tsdf", f"-Wl,-rpath,{libdir}",
+    exe = os.path.join(str(out_dir), "shim_example")
+    subprocess.run([CXX, "-std=c++17", "-O1", SRC, "-o", exe, f"-L{libdir}", "-lb200tsdf", f"-Wl,-rpath,{libdir}",
                     "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"], check=True)
-    return EXE
+    return exe
 
 
-def test_shim_compiles_and_reports_missing_device(engine_lib):
-    exe = build(engine_lib)
+def test_shim_compiles_and_reports_missing_device(engine_lib, tmp_path):
+    exe = build(engine_lib, tmp_path)
     try:
         import torch
         if torch.cuda.is_available():
@@ -31,8 +31,8 @@ def test_shim_compiles_and_reports_missing_device(engine_lib):
 
 
 @pytest.mark.gpu
-def test_shim_example_runs(engine_lib):
-    exe = build(engine_lib)
+def test_shim_example_runs(engine_lib, tmp_path):
+    exe = build(engine_lib, tmp_path)
     r = subprocess.run([exe], capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "mesh:" in r.stdout

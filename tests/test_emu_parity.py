@@ -71,6 +71,10 @@ def test_other_tier_shapes(res, size, cell):
         assert np.array_equal(a[3], b[3])
         for k in range(3):
             assert np.array_equal(a[k][a[3]], b[k][b[3]])
+    # the mesh's brick walk, triangle for triangle in the reference's order (w_min 0: two frames leave weights of at most 2)
+    va, _ = o.mesh(0.0, 0); vb, _ = e.mesh(0.0, 0)
+    assert len(va) == len(vb) > 0
+    assert np.array_equal(np.asarray(va).view(np.uint32), np.asarray(vb).view(np.uint32))
 
 
 def test_edge_cases_empty_nan_and_out_of_volume():

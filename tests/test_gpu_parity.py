@@ -111,6 +111,14 @@ def test_other_tier_shapes(res, size, cell):
     for pose, cloud in frames(scene, 2, stride=6, noise_seed=9):
         o.integrate(cloud, pose); e.integrateCloud(cloud, None, pose)
     assert_same_nodes(o.dump_nodes(), e.download_nodes())
+    # the mesh's brick walk, triangle for triangle in the reference's order (w_min 0: two frames leave weights of at most 2)
+    mc = pkg.MarchingCubesTSDFOctree()
+    mc.setInputTSDF(e)
+    mc.setMinWeight(0.0)
+    vb, _, _ = mc.reconstruct()
+    va, _ = o.mesh(0.0, 0)
+    assert len(va) == len(vb) > 0
+    assert np.array_equal(np.asarray(va).view(np.uint32), np.asarray(vb).reshape(-1, 3).view(np.uint32))
 
 
 def test_edge_cases_empty_nan_and_out_of_volume():
