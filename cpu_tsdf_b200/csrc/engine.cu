@@ -940,9 +940,11 @@ int b200tsdf_reset (b200tsdf_t* h)
   }
   {
     // work queues for levels C .. B = L-3 (fast path needs the block-root level at or below the coarse depth)
+    // the brick kernels divide with div_recip / div_with, which equal __fdiv_rn only inside Params::exact_div_ok; other
+    // truncation limits and weight caps are fused by the general depth-first kernel, which uses the IEEE division
     int Bl = np.L - 3;
     h->force_general = c.debug_flags & 1;
-    h->fast_path = (Bl >= np.C) && !var && !np.color_norm && !h->force_general && (Bl - np.C + 1 <= MAX_QLEVELS);
+    h->fast_path = (Bl >= np.C) && !var && !np.color_norm && !h->force_general && np.exact_div_ok && (Bl - np.C + 1 <= MAX_QLEVELS);
     h->q_levels = h->fast_path ? (Bl - np.C + 1) : 0;
     size_t total = 0; size_t caps[MAX_QLEVELS] = {};
     for (int i = 0; i < h->q_levels; ++i)

@@ -55,8 +55,11 @@ inline const char* derive_params (const b200tsdf_config& c, Params& p, size_t& p
     const double M = std::max (c.image_width, c.image_height) + 2.0, cc = std::max (std::fabs (c.cx), std::fabs (c.cy));
     p.proj_guard = (float) (1.5 * ((M + cc) * std::ldexp (1.0, -22) + M * std::ldexp (1.0, -24)));
     if (!(p.proj_guard < 0.05f)) p.fast_proj = 0;
+    // the operands of the brick kernels' divisions (div_with): d_new, clamped to [-max_dist_neg, max_dist_pos], over
+    // max_dist_neg; the weighted sums over w + 1 <= max_weight + 1.  The sensor bounds are not among them, so the
+    // integrate program's default min_sensor_dist = 0 keeps the brick kernels.
     p.exact_div_ok = (c.max_dist_neg >= 1e-6f && c.max_dist_neg <= 1e6f && std::fabs (c.max_dist_pos) <= 1e6f
-                      && c.max_weight >= 0.f && c.max_weight <= 1e9f && c.min_sensor_dist >= 1e-6f && c.max_sensor_dist <= 1e6f) ? 1 : 0;
+                      && c.max_weight >= 0.f && c.max_weight <= 1e9f) ? 1 : 0;
   }
   p.color = c.integrate_color != 0; p.track_var = c.track_variance != 0;
   if (c.color_mode == B200TSDF_COLOR_LAB)

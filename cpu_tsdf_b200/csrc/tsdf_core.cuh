@@ -140,7 +140,7 @@ struct Params
   // (double) d < t  <=>  d < (smallest float >= t)
   float rc_lo_f, rc_hi_f;         // thresholds -0.99 and rc_thresh of the return code (hpp:209-214)
   float proj_guard;               // half-width of the band around an integer inside which the float pixel estimate is not trusted
-  int exact_div_ok;               // 1 when every divisor of the update lies where __fdiv_rn takes its fast path (see div_with)
+  int exact_div_ok;               // 1 when every divisor of the update lies where __fdiv_rn takes its fast path (see div_with); the brick kernels run only then
   int width, height;
   int color, track_var;
   int color_norm;                 // colour payload is RGBNormalized (setColorMode ("RGBNormalized"), octree.cpp:379-434) instead of RGB
