@@ -496,7 +496,7 @@ __global__ void __launch_bounds__ (TOP_THREADS) k_celltop_down (Params p, const 
   const double thr[4] = { near_threshold (sizeC), near_threshold (sizeC * 0.5f), near_threshold (sizeC * 0.25f), near_threshold (sizeC * 0.125f) };
   const float thrf[4] = { float_at_least (thr[0]), float_at_least (thr[1]), float_at_least (thr[2]), float_at_least (thr[3]) };
   const bool have_bgra = COLOR && p.color && f.rgba_off >= 0;
-  FrameHot F; F.pts = f.pts + f.xyz_off + 8; F.stride = f.stride; F.coff = have_bgra ? f.rgba_off - (f.xyz_off + 8) : 0;
+  FrameHot F; F.pix = p.pix;
   for (int ci = blockIdx.x; ci < count; ci += gridDim.x)
   {
     __syncthreads ();

@@ -142,6 +142,51 @@ __global__ void k_front (Params p, const FrameRec* __restrict__ fr, int cull_blo
 {
   pdl_launch_dependents ();
   B2_STAGE_FRAME (fr)
+  // what depends only on the frame and the caller's cloud is done before waiting for the previous frame: the frustum test
+  // of a coarse cell, and a pixel's point load, world transform and descent to its finest voxel.  The blocks that are
+  // resident while the previous frame's bottom-up sweep drains so hide the cloud's DRAM latency behind it.
+  const bool cull = (int) blockIdx.x < cull_blocks;
+  const int n = 1 << p.C;
+  int i, x = 0, y = 0, z = 0;
+  bool act;                                             // cull: the cell is culled in and owned; pixel: inside the image
+  bool split_it = false;                                // pixel: its finest voxel is in the volume and in an owned cell
+  int fx_ = 0, fy_ = 0, fz_ = 0;
+  uint32_t zb = 0u, bgra = 0u;
+  if (cull)
+  {
+    i = blockIdx.x * blockDim.x + threadIdx.x;
+    act = i < n * n * n;
+    if (act)
+    {
+      z = i % n; y = (i / n) % n; x = i / (n * n);
+      const float cx = center1d (p, p.C, x), cy = center1d (p, p.C, y), cz = center1d (p, p.C, z);
+      act = frustum_contains (s_fr_.pl, cx, cy, cz) && owns_cell (p, x, y, z);
+    }
+  }
+  else
+  {
+    i = (blockIdx.x - cull_blocks) * blockDim.x + threadIdx.x;
+    act = i < f.width * f.height;
+    if (act)
+    {
+      const int u = i % f.width, v = i / f.width;
+      const float* pt = frame_xyz (f, u, v);
+      zb = reinterpret_cast<const uint32_t*> (pt)[2];
+      if (p.color && f.rgba_off >= 0) bgra = *reinterpret_cast<const uint32_t*> (frame_bgr (f, u, v));
+      const float zf = __uint_as_float (zb);
+      if (!is_nan (zf))                                                 // hpp:64
+      {
+        float pw[3];
+        affine_mul_f (f.tfwd, pt[0], pt[1], zf, pw);                    // hpp:76
+        split_it = world_to_finest (p, pw[0], pw[1], pw[2], fx_, fy_, fz_);
+        if (split_it && p.shard_count > 1)
+        {
+          const int sh = p.L - p.C;
+          split_it = owns_cell (p, fx_ >> sh, fy_ >> sh, fz_ >> sh);
+        }
+      }
+    }
+  }
   pdl_wait ();                                          // the previous frame's bottom-up sweep has finished
   int* count = d_count + 16 * s_fr_.cset;
   int* next_counts = d_count + 16 * (s_fr_.cset ^ 1);
@@ -152,14 +197,9 @@ __global__ void k_front (Params p, const FrameRec* __restrict__ fr, int cull_blo
     if (threadIdx.x < ST_N) stats[ST_N + threadIdx.x] = stats[threadIdx.x];
     next_counts[threadIdx.x] = 0;
   }
-  if ((int) blockIdx.x < cull_blocks)
+  if (!act) return;
+  if (cull)
   {
-    int n = 1 << p.C;
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n * n * n) return;
-    int z = i % n, y = (i / n) % n, x = i / (n * n);
-    float cx = center1d (p, p.C, x), cy = center1d (p, p.C, y), cz = center1d (p, p.C, z);
-    if (!frustum_contains (s_fr_.pl, cx, cy, cz) || !owns_cell (p, x, y, z)) return;
     int k = atomicAdd (count, 1);
     list[k] = i;
     if (q0)
@@ -171,22 +211,12 @@ __global__ void k_front (Params p, const FrameRec* __restrict__ fr, int cull_blo
     }
     return;
   }
-  int i = (blockIdx.x - cull_blocks) * blockDim.x + threadIdx.x;
-  if (i >= f.width * f.height) return;
-  int u = i % f.width, v = i / f.width;
-  const float* pt = frame_xyz (f, u, v);
-  float z = pt[2];
-  if (is_nan (z)) return;                                        // hpp:64
-  float pw[3];
-  affine_mul_f (f.tfwd, pt[0], pt[1], z, pw);                    // hpp:76
-  int fx_, fy_, fz_;
-  if (!world_to_finest (p, pw[0], pw[1], pw[2], fx_, fy_, fz_)) return;
-  if (p.shard_count > 1)
-  {
-    int sh = p.L - p.C;
-    if (!owns_cell (p, fx_ >> sh, fy_ >> sh, fz_ >> sh)) return;
-  }
-  presplit_point (p, fx_, fy_, fz_);
+  // the pixel plane the observations of this frame read (Params::pix): a bit copy of every pixel, NaN depths, points
+  // outside the volume and points in another shard's cells included, because an observation may project onto any pixel.
+  // Written only past pdl_wait: the previous frame's readers are done.
+  if (p.color) reinterpret_cast<uint2*> (p.pix)[i] = make_uint2 (zb, bgra);
+  else p.pix[i] = zb;
+  if (split_it) presplit_point (p, fx_, fy_, fz_);
 }
 
 // general path: one thread per culled coarse cell runs updateVoxel depth-first
@@ -564,6 +594,7 @@ struct b200tsdf
   int count_set = 0;             // which of the two per-frame counter sets the last frame used
   int* d_culled = nullptr; int* d_count = nullptr; unsigned long long* d_stats = nullptr;
   size_t culled_cap = 0;
+  uint32_t* d_pix = nullptr; size_t pix_cap = 0;   // Params::pix (bytes allocated, grow-only)
   bool timed = false;
   bool time_frames = false;      // set between profile_begin / profile_end: per-frame event records (ev_t0/ev_t1 and the ring around the dominant kernel)
   bool is_empty = true;          // TSDFVolumeOctree::is_empty_ (cpp:205, hpp:101)
@@ -846,7 +877,7 @@ void b200tsdf_destroy (b200tsdf_t* h)
   if (h->copy_stream) cudaStreamSynchronize (h->copy_stream);
   if (h->gather_stream) cudaStreamSynchronize (h->gather_stream);
   free_volume (h);
-  cudaFree (h->d_err); cudaFree (h->d_count); cudaFree (h->d_stats); cudaFree (h->d_culled); cudaFree (h->d_scratch);
+  cudaFree (h->d_err); cudaFree (h->d_count); cudaFree (h->d_stats); cudaFree (h->d_culled); cudaFree (h->d_pix); cudaFree (h->d_scratch);
   cudaFree (h->d_dbg); if (h->h_err) cudaFreeHost (h->h_err);
   cudaFree (h->d_params); cudaFree (h->d_ring); if (h->h_ring) cudaFreeHost (h->h_ring);
   for (int i = 0; i < 2; ++i) if (h->ev_ring[i]) cudaEventDestroy (h->ev_ring[i]);
@@ -938,6 +969,14 @@ int b200tsdf_reset (b200tsdf_t* h)
     CK (cudaMalloc (&h->d_culled, ncells * sizeof (int)));
     h->culled_cap = ncells;
   }
+  const size_t pix_bytes = (size_t) np.width * np.height * (color ? 8 : 4);
+  if (pix_bytes > h->pix_cap)
+  {
+    h->has_volume = false;                                 // the frames' launches need the plane
+    cudaFree (h->d_pix); h->d_pix = nullptr; h->pix_cap = 0; h->p.pix = nullptr;
+    CK (cudaMalloc (&h->d_pix, pix_bytes));
+    h->pix_cap = pix_bytes;
+  }
   {
     // work queues for levels C .. B = L-3 (fast path needs the block-root level at or below the coarse depth)
     // the brick kernels divide with div_recip / div_with, which equal __fdiv_rn only inside Params::exact_div_ok; other
@@ -1011,6 +1050,7 @@ int b200tsdf_reset (b200tsdf_t* h)
     p.rgbn = st.rgbn; p.root_rgbn = st.root_rgbn;
   }
   p.err = h->d_err;
+  p.pix = h->d_pix;
   p.diag = h->d_stats + 3;
   p.dbg = h->d_dbg;
   CK (cudaMemcpyAsync (h->d_params, &p, sizeof (Params), cudaMemcpyHostToDevice, h->stream));
