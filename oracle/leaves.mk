@@ -20,7 +20,7 @@ REF_SRCS := $(REF)/src/lib/octree.cpp $(REF)/src/lib/tsdf_volume_octree.cpp \
 
 ref: $(HERE)_ref/libcpu_tsdf_ref_leaves.so
 
-$(HERE)_ref/libcpu_tsdf_ref_leaves.so: $(HERE)ref_leaves_capi.cpp $(HERE)tsdf_oracle_leaves.h $(HERE)ref_capi.cpp $(wildcard $(HERE)compat/*/*.h $(HERE)compat/*/*/*.h $(HERE)compat/*/*/*/*.h*) $(HERE)ref_arith.h $(HERE)mc_tables.h
+$(HERE)_ref/libcpu_tsdf_ref_leaves.so: $(HERE)ref_leaves_capi.cpp $(HERE)tsdf_oracle_leaves.h $(HERE)ref_capi.cpp $(HERE)tsdf_oracle.h $(wildcard $(HERE)compat/*/*.h $(HERE)compat/*/*/*.h $(HERE)compat/*/*/*/*.h*) $(HERE)ref_arith.h $(HERE)mc_tables.h
 	@test -d $(REF) || (echo "reference tree $(REF) not present: skipping oracle/_ref" && false)
 	mkdir -p $(HERE)_ref
 	$(CXX) $(CXXFLAGS) -Wno-reorder -Wno-sign-compare -Wno-unused-but-set-variable -Wno-deprecated-declarations \

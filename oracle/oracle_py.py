@@ -36,6 +36,7 @@ class OrcStats(C.Structure):
         ("n_add_observation", C.c_int64), ("n_node_visits", C.c_int64), ("n_presplit", C.c_int64),
         ("n_culled_cells", C.c_int64), ("n_nodes", C.c_int64),
         ("t_presplit", C.c_double), ("t_cull", C.c_double), ("t_update", C.c_double),
+        ("n_prune_existing", C.c_int64), ("n_prune_resplit", C.c_int64),
     ]
 
 

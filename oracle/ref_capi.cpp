@@ -124,6 +124,7 @@ int orc_integrate (orc_volume* v, const void* points, size_t stride, int xyz_off
   std::memset (&v->stats, 0, sizeof (v->stats));
   v->stats.t_update = t1 - t0;          // integrateCloud only (the reference has no per-phase timers)
   v->stats.n_add_observation = -1; v->stats.n_node_visits = -1; v->stats.n_presplit = -1; v->stats.n_culled_cells = -1; v->stats.n_nodes = -1;
+  v->stats.n_prune_existing = -1; v->stats.n_prune_resplit = -1;
   return 0;
 }
 

@@ -98,7 +98,7 @@ inline int thread_id ()
 #endif
 }
 
-struct PerThread { int64_t n_add = 0, n_visit = 0; char pad[48]; };
+struct PerThread { int64_t n_add = 0, n_visit = 0, n_prune = 0, n_resplit = 0; char pad[32]; };
 
 } // namespace
 
@@ -278,6 +278,7 @@ struct orc_volume
   int update_voxel (int32_t ni, const Frame& f, int tid)
   {
     pt[tid].n_visit++;
+    bool pruned = false;                                          // (event counter only: the pre-existing children were pruned)
     if (pool.at (ni).child >= 0)                                  // hpp:122-142
     {
       int32_t first = pool.at (ni).child;
@@ -285,6 +286,8 @@ struct orc_volume
       for (int i = 0; i < 8; ++i) all_are_empty &= (update_voxel (first + i, f, tid) < 0);
       if (all_are_empty) { pool.free8 (first, tid); pool.at (ni).child = -1; }
       else return 1;
+      pt[tid].n_prune++;
+      pruned = true;
     }
     Node& n = pool.at (ni);
     float ctr[3] = { n.cx, n.cy, n.cz }, v_g[3];
@@ -300,6 +303,7 @@ struct orc_volume
     {
       if (n.size > c.xsize / c.xres && n.size > c.ysize / c.yres && n.size > c.zsize / c.zres)   // hpp:165
       {
+        if (pruned) pt[tid].n_resplit++;
         int32_t first = split (ni, tid);
         bool all_are_empty = true;
         for (int i = 0; i < 8; ++i) all_are_empty &= (update_voxel (first + i, f, tid) < 0);
@@ -474,7 +478,7 @@ int orc_integrate (orc_volume* v, const void* points, size_t stride, int xyz_off
   affine_inverse (pose, inv);                                     // hpp:54
   float trans_f[16];
   for (int i = 0; i < 16; ++i) { f.trans_inv[i] = static_cast<float> (inv[i]); trans_f[i] = static_cast<float> (pose[i]); }
-  for (auto& p : v->pt) { p.n_add = 0; p.n_visit = 0; }
+  for (auto& p : v->pt) { p.n_add = 0; p.n_visit = 0; p.n_prune = 0; p.n_resplit = 0; }
 
   double t0 = now_s ();
   int64_t nsplit = 0;
@@ -517,8 +521,12 @@ int orc_integrate (orc_volume* v, const void* points, size_t stride, int xyz_off
 
   v->is_empty = false;                                            // hpp:101
   orc_stats& s = v->stats;
-  s.n_add_observation = 0; s.n_node_visits = 0;
-  for (auto& p : v->pt) { s.n_add_observation += p.n_add; s.n_node_visits += p.n_visit; }
+  s.n_add_observation = 0; s.n_node_visits = 0; s.n_prune_existing = 0; s.n_prune_resplit = 0;
+  for (auto& p : v->pt)
+  {
+    s.n_add_observation += p.n_add; s.n_node_visits += p.n_visit;
+    s.n_prune_existing += p.n_prune; s.n_prune_resplit += p.n_resplit;
+  }
   s.n_presplit = nsplit; s.n_culled_cells = static_cast<int64_t> (culled.size ());
   s.n_nodes = v->pool.live.load ();
   s.t_presplit = t1 - t0; s.t_cull = t2 - t1; s.t_update = t3 - t2;

@@ -60,6 +60,8 @@ typedef struct orc_stats
   int64_t n_culled_cells;      /* coarse cells kept by the frustum cull */
   int64_t n_nodes;             /* live nodes in the tree               */
   double t_presplit, t_cull, t_update;  /* seconds */
+  int64_t n_prune_existing;    /* nodes whose children, present before this frame, were all pruned (hpp:136-141) */
+  int64_t n_prune_resplit;     /* of those, nodes that split again in the same updateVoxel call (hpp:161-165) */
 } orc_stats;
 void orc_get_stats (const orc_volume* v, orc_stats* s);
 
