@@ -73,6 +73,7 @@ EXPORTS = [
     "b200tsdf_set_config", "b200tsdf_get_config", "b200tsdf_reset", "b200tsdf_integrate",
     "b200tsdf_integrate_device", "b200tsdf_integrate_batch_device", "b200tsdf_integrate_async",
     "b200tsdf_comm_unique_id", "b200tsdf_comm_init", "b200tsdf_row_slice", "b200tsdf_integrate_batch_rows", "b200tsdf_gather_volume", "b200tsdf_sync", "b200tsdf_organize", "b200tsdf_integrate_unorganized", "b200tsdf_query", "b200tsdf_interpolate", "b200tsdf_render", "b200tsdf_mesh",
+    "b200tsdf_query_device", "b200tsdf_interpolate_device", "b200tsdf_render_batch_device",
     "b200tsdf_free", "b200tsdf_save", "b200tsdf_load", "b200tsdf_export_shard", "b200tsdf_import_shard", "b200tsdf_voxel_center", "b200tsdf_voxel_index",
     "b200tsdf_voxel_centers", "b200tsdf_occupied_voxel_indices", "b200tsdf_is_empty",
     "b200tsdf_get_stats", "b200tsdf_download_nodes", "b200tsdf_download_color_payload", "b200tsdf_frustum_cull",
@@ -121,6 +122,9 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_query.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.b200tsdf_interpolate.argtypes = [vp, vp, C.c_int, vp, vp]
     lib.b200tsdf_render.argtypes = [vp, vp, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, vp]
+    lib.b200tsdf_query_device.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
+    lib.b200tsdf_interpolate_device.argtypes = [vp, vp, C.c_int, vp, vp]
+    lib.b200tsdf_render_batch_device.argtypes = [vp, C.c_int, vp, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, vp]
     lib.b200tsdf_mesh.argtypes = [vp, C.c_float, C.c_int, C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_size_t)]
     lib.b200tsdf_save.argtypes = [vp, C.c_char_p]
     lib.b200tsdf_load.argtypes = [vp, C.c_char_p]
@@ -425,6 +429,32 @@ class TSDFVolumeOctree:
         pose = _pose(trans)
         self._check(self._lib.b200tsdf_render(self._h, _ptr(pose), downsampleBy, _ptr(out), 48, 0, 16, _ptr(rgb)))
         return out, rgb
+
+    # ---- reads into device memory: buffers are integer device pointers on this handle's device (e.g. a torch tensor's
+    # data_ptr()); the calls are asynchronous on the handle's stream, ordered after earlier integrates (sync() before reading)
+    def renderViewBatchDevice(self, poses, d_out: int, stride: int = 48, xyz_off: int = 0, normal_off: int = 16,
+                              d_rgb: int | None = None, downsampleBy: int = 1) -> bool:
+        """renderView (renderColoredView with d_rgb) for every pose: pose i's (H/ds) x (W/ds) image starts at
+        d_out + i * (H/ds) * (W/ds) * stride; xyz at xyz_off and the normal at normal_off are the only bytes written;
+        d_rgb takes 3 bytes per pixel."""
+        ps = np.ascontiguousarray(np.stack([_pose(t) for t in poses]) if len(poses) else np.zeros((0, 4, 4)), dtype=np.float64)
+        self._check(self._lib.b200tsdf_render_batch_device(self._h, len(ps), _ptr(ps), downsampleBy, C.c_void_p(int(d_out)), stride,
+                                                           xyz_off, normal_off, None if d_rgb is None else C.c_void_p(int(d_rgb))))
+        return True
+
+    def queryDevice(self, d_xyz: int, n: int, d_ok: int, what: int = 1, mode: int = 0, d_val: int | None = None,
+                    d_grad: int | None = None, d_hess: int | None = None) -> bool:
+        """getFxn / getGradient / getHessian (mode 0) or the combined forms (mode 1) at n device points (3 floats each),
+        like getFxn & co.: what bit0 value (1 float), bit1 gradient (3), bit2 hessian (9); d_ok[i] = the reference's bool."""
+        dp = lambda a: None if a is None else C.c_void_p(int(a))
+        self._check(self._lib.b200tsdf_query_device(self._h, dp(d_xyz), n, what, mode, dp(d_val), dp(d_grad), dp(d_hess), dp(d_ok)))
+        return True
+
+    def getTSDFValueDevice(self, d_xyz: int, n: int, d_val: int, d_valid: int) -> bool:
+        """getTSDFValue at n device points: d_valid (uint8) holds the caller's flags on entry and is only ever cleared."""
+        dp = lambda a: None if a is None else C.c_void_p(int(a))
+        self._check(self._lib.b200tsdf_interpolate_device(self._h, dp(d_xyz), n, dp(d_val), dp(d_valid)))
+        return True
 
     def save(self, filename: str):
         """cpp:222-245"""

@@ -81,6 +81,8 @@ enum StatSlot { ST_UPDATES = 0, ST_VISITS = 1, ST_BLOCKS = 2, ST_N = 8, ST_TOTAL
 constexpr int KRING = 64;     // ring of event pairs around the dominant kernel
 constexpr int FRAME_RING = 64;  // per-frame records in flight (device ring + its pinned host image)
 constexpr int BATCH_SEGS = 16;  // host staging segments of the batch path
+constexpr int RENDER_CHUNK = 32;  // poses per render launch (blockIdx.z)
+constexpr int RENDER_SEGS = 8;    // pinned staging segments of RENDER_CHUNK render records
 
 // ---------------------------------------------------------------------------------------------
 // kernels
@@ -250,8 +252,8 @@ __global__ void k_query (Params gp, const float* __restrict__ xyz, int n, int wh
                          float* val, float* grad, float* hess, unsigned char* ok)
 {
   B2_STAGE_PARAMS (gp)
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  const size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t) n) return;
   float v, g[3], hs[9];
   bool good = query_point (p, xyz + 3 * i, mode, &v, g, hs);
   ok[i] = good ? 1 : 0;
@@ -265,25 +267,35 @@ __global__ void k_query (Params gp, const float* __restrict__ xyz, int n, int wh
 __global__ void k_interpolate (Params gp, const float* __restrict__ xyz, int n, float* __restrict__ val, unsigned char* __restrict__ valid)
 {
   B2_STAGE_PARAMS (gp)
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+  const size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t) n) return;
   bool v = valid[i] != 0;
   val[i] = interpolate_trilinearly (p, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], &v);
   valid[i] = v ? 1 : 0;
 }
 
-__global__ void k_render (Params gp, RenderParams r, float* __restrict__ out /* 6 floats per pixel */, unsigned char* __restrict__ rgb)
+// renderView for a batch of poses: blockIdx.z is the pose within the launch, and each block stages that pose's record.  Pixels
+// are row-major, one image after the other; each gets 12 bytes of xyz at xyz_off and 12 of normal at normal_off (4-byte
+// aligned), and no other byte of the caller's buffer is written.  rgb: 3 bytes per pixel, or null.
+__global__ void k_render (Params gp, const RenderParams* __restrict__ recs, unsigned char* __restrict__ out, size_t stride,
+                          int xyz_off, int normal_off, unsigned char* __restrict__ rgb)
 {
-  B2_STAGE_PARAMS (gp)
+  __shared__ RenderParams sr_;
+  for (int w = threadIdx.x; w < (int) (sizeof (RenderParams) / sizeof (int)); w += blockDim.x)
+    reinterpret_cast<int*> (&sr_)[w] = reinterpret_cast<const int*> (recs + blockIdx.z)[w];
+  B2_STAGE_PARAMS (gp)                                  // (its barrier also covers the record)
+  const RenderParams& r = sr_;
   // 8x8 pixel tiles keep neighbouring rays in one warp-pair
   int tx = threadIdx.x % 8, ty = threadIdx.x / 8;
   int x = blockIdx.x * 8 + tx, y = blockIdx.y * 8 + ty;
   if (x >= r.width || y >= r.height) return;
-  size_t i = (size_t) y * r.width + x;
+  const size_t i = ((size_t) blockIdx.z * r.height + y) * r.width + x;
   float P[3], N[3];
   render_pixel (p, r, x, y, P, N, rgb ? rgb + 3 * i : nullptr);
-  float* o = out + 6 * i;
-  o[0] = P[0]; o[1] = P[1]; o[2] = P[2]; o[3] = N[0]; o[4] = N[1]; o[5] = N[2];
+  float* o = reinterpret_cast<float*> (out + i * stride + xyz_off);
+  o[0] = P[0]; o[1] = P[1]; o[2] = P[2];
+  o = reinterpret_cast<float*> (out + i * stride + normal_off);
+  o[0] = N[0]; o[1] = N[1]; o[2] = N[2];
 }
 
 __global__ void k_list_bricks (Params p, int* __restrict__ list, int* __restrict__ count)
@@ -660,6 +672,10 @@ struct b200tsdf
   void* leaf_xyz = nullptr; void* leaf_ijk = nullptr;       // b200tsdf_voxel_centers / _occupied_voxel_indices results
   // grow-only device scratch for the read-side calls (queries, render): no allocation per call
   unsigned char* d_scratch = nullptr; size_t scratch_cap = 0;
+  // render records (b200tsdf_render_batch_device), allocated at the first render: one device chunk, reused in stream order,
+  // and RENDER_SEGS pinned staging segments written round robin, each free again once the copy that read it has run
+  RenderParams* d_rrec = nullptr; RenderParams* h_rrec = nullptr; int rrec_seg = 0; bool rrec_used[RENDER_SEGS] = {};
+  cudaEvent_t ev_rrec[RENDER_SEGS] = {};
   int scratch (size_t bytes)
   {
     if (bytes <= scratch_cap) return 0;
@@ -892,6 +908,8 @@ void b200tsdf_destroy (b200tsdf_t* h)
     if (h->ev_rows_done[i]) cudaEventDestroy (h->ev_rows_done[i]);
   }
   cudaFree (h->d_bring); if (h->h_bring) cudaFreeHost (h->h_bring);
+  cudaFree (h->d_rrec); if (h->h_rrec) cudaFreeHost (h->h_rrec);
+  for (int i = 0; i < RENDER_SEGS; ++i) if (h->ev_rrec[i]) cudaEventDestroy (h->ev_rrec[i]);
   for (int i = 0; i < BATCH_SEGS; ++i) if (h->ev_bring[i]) cudaEventDestroy (h->ev_bring[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_half_done[i]) cudaEventDestroy (h->ev_half_done[i]);
   cudaFree (h->d_frame[0]); cudaFree (h->d_frame[1]); cudaFree (h->q_mem); cudaFree (h->d_blist); cudaFree (h->d_bail); cudaFree (h->d_cellq); cudaFree (h->d_superq); cudaFree (h->d_celltop);
@@ -1558,12 +1576,31 @@ int b200tsdf_get_stats (b200tsdf_t* h, b200tsdf_stats* s)
 }
 
 // ---- point queries (tsdf_volume_octree.cpp:655-794) -------------------------------------------------
-int b200tsdf_query (b200tsdf_t* h, const float* xyz, int n, int what, int mode,
-                    float* val, float* grad, float* hess, uint8_t* ok)
+static int query_args (b200tsdf* h, const float* xyz, int n, int what, const float* val, const float* grad, const float* hess, const uint8_t* ok)
 {
   if (!h || !xyz || !ok || n < 0) return B200TSDF_EINVAL;
   if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "query before reset()");
   if (((what & 1) && !val) || ((what & 2) && !grad) || ((what & 4) && !hess)) return h->fail (B200TSDF_EINVAL, "missing output buffer");
+  return B200TSDF_OK;
+}
+
+int b200tsdf_query_device (b200tsdf_t* h, const float* d_xyz, int n, int what, int mode,
+                           float* d_val, float* d_grad, float* d_hess, uint8_t* d_ok)
+{
+  if (int rc = query_args (h, d_xyz, n, what, d_val, d_grad, d_hess, d_ok)) return rc;
+  if (n == 0) return B200TSDF_OK;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  k_query<<<(n + 127) / 128, 128, 0, h->stream>>> (h->p, d_xyz, n, what, mode, d_val, d_grad, d_hess, d_ok);
+  CK (cudaGetLastError ());
+  note_device_err (h, h->stream);
+  return B200TSDF_OK;
+}
+
+int b200tsdf_query (b200tsdf_t* h, const float* xyz, int n, int what, int mode,
+                    float* val, float* grad, float* hess, uint8_t* ok)
+{
+  if (int rc = query_args (h, xyz, n, what, val, grad, hess, ok)) return rc;
   if (n == 0) return B200TSDF_OK;
   cudaSetDevice (h->device);
   // one scratch block: xyz (12n) | val (4n) | grad (12n) | hess (36n) | ok (n)
@@ -1575,7 +1612,7 @@ int b200tsdf_query (b200tsdf_t* h, const float* xyz, int n, int what, int mode,
   unsigned char* d_ok = (unsigned char*) (d_hess + (size_t) 9 * n);
   cudaStream_t s = h->stream;
   CK (cudaMemcpyAsync (d_xyz, xyz, (size_t) n * 12, cudaMemcpyHostToDevice, s));
-  k_query<<<(n + 127) / 128, 128, 0, s>>> (h->p, d_xyz, n, what, mode, d_val, d_grad, d_hess, d_ok);
+  if (int rc = b200tsdf_query_device (h, d_xyz, n, what, mode, d_val, d_grad, d_hess, d_ok)) return rc;
   CK (cudaMemcpyAsync (ok, d_ok, (size_t) n, cudaMemcpyDeviceToHost, s));
   if (what & 1) CK (cudaMemcpyAsync (val, d_val, (size_t) n * 4, cudaMemcpyDeviceToHost, s));
   if (what & 2) CK (cudaMemcpyAsync (grad, d_grad, (size_t) n * 12, cudaMemcpyDeviceToHost, s));
@@ -1586,6 +1623,19 @@ int b200tsdf_query (b200tsdf_t* h, const float* xyz, int n, int what, int mode,
 }
 
 // ---- getTSDFValue / interpolateTrilinearly (tsdf_volume_octree.cpp:454-541) ---------------------------------
+int b200tsdf_interpolate_device (b200tsdf_t* h, const float* d_xyz, int n, float* d_val, uint8_t* d_valid_in_out)
+{
+  if (!h || !d_xyz || !d_val || !d_valid_in_out || n < 0) return B200TSDF_EINVAL;
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "getTSDFValue before reset()");
+  if (n == 0) return B200TSDF_OK;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  k_interpolate<<<(n + 127) / 128, 128, 0, h->stream>>> (h->p, d_xyz, n, d_val, d_valid_in_out);
+  CK (cudaGetLastError ());
+  note_device_err (h, h->stream);
+  return B200TSDF_OK;
+}
+
 int b200tsdf_interpolate (b200tsdf_t* h, const float* xyz, int n, float* val, uint8_t* valid_in_out)
 {
   if (!h || !xyz || !val || !valid_in_out || n < 0) return B200TSDF_EINVAL;
@@ -1599,7 +1649,7 @@ int b200tsdf_interpolate (b200tsdf_t* h, const float* xyz, int n, float* val, ui
   cudaStream_t s = h->stream;
   CK (cudaMemcpyAsync (d_xyz, xyz, (size_t) n * 12, cudaMemcpyHostToDevice, s));
   CK (cudaMemcpyAsync (d_ok, valid_in_out, (size_t) n, cudaMemcpyHostToDevice, s));
-  k_interpolate<<<(n + 127) / 128, 128, 0, s>>> (h->p, d_xyz, n, d_val, d_ok);
+  if (int rc = b200tsdf_interpolate_device (h, d_xyz, n, d_val, d_ok)) return rc;
   CK (cudaMemcpyAsync (val, d_val, (size_t) n * 4, cudaMemcpyDeviceToHost, s));
   CK (cudaMemcpyAsync (valid_in_out, d_ok, (size_t) n, cudaMemcpyDeviceToHost, s));
   note_device_err (h, s);
@@ -1608,27 +1658,76 @@ int b200tsdf_interpolate (b200tsdf_t* h, const float* xyz, int n, float* val, ui
 }
 
 // ---- renderView / renderColoredView (tsdf_volume_octree.cpp:278-450) ----------------------------------
+static int render_args (b200tsdf* h, int downsample, size_t stride, int xyz_off, int normal_off)
+{
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "renderView before reset()");
+  if (stride < 12 || xyz_off < 0 || normal_off < 0 || (size_t) xyz_off + 12 > stride || (size_t) normal_off + 12 > stride)
+    return h->fail (B200TSDF_EINVAL, "bad output point layout (need xyz_off + 12 <= stride and normal_off + 12 <= stride)");
+  if (h->p.width / downsample <= 0 || h->p.height / downsample <= 0) return h->fail (B200TSDF_EINVAL, "downsample too large");
+  return B200TSDF_OK;
+}
+
+// n poses, RENDER_CHUNK per launch: the chunk's records are built on the host (make_render_params), staged in pinned memory and
+// copied to the device in one copy ahead of the launch on the handle's stream
+static int render_enqueue (b200tsdf* h, int n, const double* poses, int downsample, unsigned char* d_out, size_t stride,
+                           int xyz_off, int normal_off, unsigned char* d_rgb)
+{
+  cudaStream_t s = h->stream;
+  if (!h->d_rrec)
+  {
+    CK (cudaMalloc (&h->d_rrec, RENDER_CHUNK * sizeof (RenderParams)));
+    CK (cudaHostAlloc (&h->h_rrec, (size_t) RENDER_SEGS * RENDER_CHUNK * sizeof (RenderParams), cudaHostAllocDefault));
+    for (int i = 0; i < RENDER_SEGS; ++i) CK (cudaEventCreateWithFlags (&h->ev_rrec[i], cudaEventDisableTiming));
+  }
+  const Params& p = h->p;
+  const int W = p.width / downsample, H = p.height / downsample;
+  const size_t npix = (size_t) W * H;
+  for (int i0 = 0; i0 < n; i0 += RENDER_CHUNK)
+  {
+    const int m = std::min (RENDER_CHUNK, n - i0), sg = h->rrec_seg;
+    if (h->rrec_used[sg]) CK (cudaEventSynchronize (h->ev_rrec[sg]));
+    RenderParams* recs = h->h_rrec + (size_t) sg * RENDER_CHUNK;
+    for (int k = 0; k < m; ++k) make_render_params (h->cfg, p, poses + 16 * (size_t) (i0 + k), downsample, recs[k]);
+    CK (cudaMemcpyAsync (h->d_rrec, recs, (size_t) m * sizeof (RenderParams), cudaMemcpyHostToDevice, s));
+    CK (cudaEventRecord (h->ev_rrec[sg], s));
+    h->rrec_used[sg] = true; h->rrec_seg = (sg + 1) % RENDER_SEGS;
+    const dim3 grid ((W + 7) / 8, (H + 7) / 8, m);
+    k_render<<<grid, 64, 0, s>>> (p, h->d_rrec, d_out + (size_t) i0 * npix * stride, stride, xyz_off, normal_off,
+                                  d_rgb ? d_rgb + (size_t) i0 * npix * 3 : nullptr);
+    CK (cudaGetLastError ());
+  }
+  return B200TSDF_OK;
+}
+
+int b200tsdf_render_batch_device (b200tsdf_t* h, int n, const double* poses_c2w, int downsample, void* d_out, size_t stride,
+                                  int xyz_off, int normal_off, uint8_t* d_rgb)
+{
+  if (!h || n < 1 || !poses_c2w || !d_out || downsample < 1) return B200TSDF_EINVAL;
+  if (int rc = render_args (h, downsample, stride, xyz_off, normal_off)) return rc;
+  if ((stride & 3) || (xyz_off & 3) || (normal_off & 3) || ((uintptr_t) d_out & 3))
+    return h->fail (B200TSDF_EINVAL, "bad output point layout (device images need 4-byte aligned d_out, stride, xyz_off and normal_off)");
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  if (int rc = render_enqueue (h, n, poses_c2w, downsample, (unsigned char*) d_out, stride, xyz_off, normal_off, d_rgb)) return rc;
+  note_device_err (h, h->stream);
+  return B200TSDF_OK;
+}
+
 int b200tsdf_render (b200tsdf_t* h, const double* pose, int downsample, void* out, size_t stride,
                      int xyz_off, int normal_off, uint8_t* rgb_out)
 {
   if (!h || !pose || !out || downsample < 1) return B200TSDF_EINVAL;
-  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "renderView before reset()");
-  if (stride < 12 || xyz_off < 0 || normal_off < 0 || (size_t) xyz_off + 12 > stride || (size_t) normal_off + 12 > stride)
-    return h->fail (B200TSDF_EINVAL, "bad output point layout (need xyz_off + 12 <= stride and normal_off + 12 <= stride)");
+  if (int rc = render_args (h, downsample, stride, xyz_off, normal_off)) return rc;
   cudaSetDevice (h->device);
-  const Params& p = h->p;
-  RenderParams r;
-  if (p.width / downsample <= 0 || p.height / downsample <= 0) return h->fail (B200TSDF_EINVAL, "downsample too large");
-  make_render_params (h->cfg, p, pose, downsample, r);
-  size_t npix = (size_t) r.width * r.height;
+  const size_t npix = (size_t) (h->p.width / downsample) * (h->p.height / downsample);
+  // a batch of one into scratch ({xyz, normal} per pixel), then only xyz and normal go into the caller's points: the other
+  // bytes keep what the caller put there
   { int rc = h->scratch (npix * 6 * sizeof (float) + npix * 3 + 64); if (rc) return rc; }
-  float* d_out = (float*) h->d_scratch;
   unsigned char* d_rgb = rgb_out ? h->d_scratch + npix * 6 * sizeof (float) : nullptr;
   cudaStream_t s = h->stream;
-  dim3 grid ((r.width + 7) / 8, (r.height + 7) / 8);
-  k_render<<<grid, 64, 0, s>>> (p, r, d_out, d_rgb);
+  if (int rc = render_enqueue (h, 1, pose, downsample, h->d_scratch, 6 * sizeof (float), 0, 3 * sizeof (float), d_rgb)) return rc;
   std::vector<float> tmp (npix * 6);
-  CK (cudaMemcpyAsync (tmp.data (), d_out, npix * 6 * sizeof (float), cudaMemcpyDeviceToHost, s));
+  CK (cudaMemcpyAsync (tmp.data (), h->d_scratch, npix * 6 * sizeof (float), cudaMemcpyDeviceToHost, s));
   if (rgb_out) CK (cudaMemcpyAsync (rgb_out, d_rgb, npix * 3, cudaMemcpyDeviceToHost, s));
   note_device_err (h, s);
   CK (cudaStreamSynchronize (s));

@@ -105,7 +105,7 @@ int  b200tsdf_integrate_batch_device (b200tsdf_t* h, int n, const void* const* d
  * b200tsdf_integrate) the buffer is already free on return.
  * Error reporting of the asynchronous entry points (integrate_device / _batch_device / _async, and integrate itself, which
  * waits for its upload only): a device-side failure of frame i (brick pool exhausted, work queue overflow) is reported by
- * the next call on the handle (integrate*, query, render) and at the latest by sync / get_stats / mesh / save. */
+ * the next call on the handle (integrate*, query*, interpolate*, render*) and at the latest by sync / get_stats / mesh / save. */
 int  b200tsdf_integrate_async (b200tsdf_t* h, const void* points, size_t stride, int xyz_off, int rgba_off,
                                int width, int height, const double* pose_c2w);
 int  b200tsdf_sync (b200tsdf_t* h);
@@ -146,12 +146,26 @@ int  b200tsdf_query (b200tsdf_t* h, const float* xyz, int n, int what, int mode,
  * its border layer; valid_in_out[i] is the caller's `*valid` on entry and is only ever cleared (border, or a neighbour with
  * weight 0), exactly like the reference's pointer argument.  Host pointers. */
 int  b200tsdf_interpolate (b200tsdf_t* h, const float* xyz, int n, float* val, uint8_t* valid_in_out);
+/* b200tsdf_query / b200tsdf_interpolate on arrays resident in device memory of h's device (every pointer is a device
+ * pointer; the same argument checks).  Asynchronous on the handle's stream, ordered after earlier integrates: call
+ * b200tsdf_sync (or order the caller's stream behind it) before reading the results.  Errors as for b200tsdf_integrate_device. */
+int  b200tsdf_query_device (b200tsdf_t* h, const float* d_xyz, int n, int what, int mode,
+                            float* d_val, float* d_grad, float* d_hess, uint8_t* d_ok);
+int  b200tsdf_interpolate_device (b200tsdf_t* h, const float* d_xyz, int n, float* d_val, uint8_t* d_valid_in_out);
 
 /* renderView (cpp:278-424) and, with rgb_out != NULL, renderColoredView (cpp:427-450).
  * out: (W/ds)*(H/ds) points of `stride` bytes; xyz at xyz_off, normal at normal_off
  * (pcl::PointNormal: 0 / 16 / 48).  Camera frame, NaN xyz = miss. */
 int  b200tsdf_render (b200tsdf_t* h, const double* pose_c2w, int downsample, void* out, size_t stride,
                       int xyz_off, int normal_off, uint8_t* rgb_out);
+/* renderView (and renderColoredView with d_rgb != NULL) for n >= 1 poses into device memory of h's device, the same pixels
+ * as n calls of b200tsdf_render.  poses_c2w: n row-major 4x4 matrices in host memory (read before the call returns).  Pose
+ * i's image starts at d_out + i*(W/ds)*(H/ds)*stride, pixels row-major; 12 bytes of xyz are written at xyz_off and 12 of
+ * normal at normal_off, no other byte (d_out, stride and both offsets 4-byte aligned).  d_rgb: 3 bytes per pixel, images
+ * back to back.  Asynchronous on the handle's stream and ordered after earlier integrates; errors as for
+ * b200tsdf_integrate_device. */
+int  b200tsdf_render_batch_device (b200tsdf_t* h, int n, const double* poses_c2w, int downsample, void* d_out, size_t stride,
+                                   int xyz_off, int normal_off, uint8_t* d_rgb);
 
 /* MarchingCubesTSDFOctree::performReconstruction (src/lib/marching_cubes_tsdf_octree.cpp:
  * 108-143): triangle soup, 3 vertices per triangle, global transform applied.
