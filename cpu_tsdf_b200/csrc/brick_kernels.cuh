@@ -116,7 +116,7 @@ __device__ __forceinline__ void warp_add_stats (unsigned long long* stats, unsig
 // brick slot instead of having their children queued.
 // The frame comes from its record in device memory and the counters from the record's counter set (Q.n = the base of all
 // sets), so that the launch can be captured into a graph and replayed like the other kernels of a frame.
-#define B2_UPPER_FRAME(fr)                                                                   \
+#define B2_SHARED_FRAME(fr)                                                                  \
   __shared__ Frame s_uf_;                                                                    \
   {                                                                                          \
     const int* src_ = reinterpret_cast<const int*> (&(fr)->f);                               \
@@ -124,7 +124,9 @@ __device__ __forceinline__ void warp_add_stats (unsigned long long* stats, unsig
     for (int w_ = threadIdx.x; w_ < (int) (sizeof (Frame) / sizeof (int)); w_ += blockDim.x) dst_[w_] = src_[w_]; \
   }                                                                                          \
   __syncthreads ();                                                                          \
-  const Frame& f = s_uf_;                                                                    \
+  const Frame& f = s_uf_;
+#define B2_UPPER_FRAME(fr)                                                                   \
+  B2_SHARED_FRAME (fr)                                                                       \
   int* const qn = Q.n + 16 * (fr)->cset;
 
 __global__ void k_upper_down (Params p, const FrameRec* __restrict__ fr, Queues Q, int li, int block_level, int* __restrict__ blist,
@@ -246,15 +248,6 @@ __global__ void k_upper_up (Params p, const FrameRec* __restrict__ fr, Queues Q,
 }
 
 // ---- helpers of the bottom-up sweeps ---------------------------------------------------------------------------
-// fold the children's return codes into an interior node (hpp:131-142 / :176-188 + fall-through)
-__device__ __noinline__ int upper_fold_slow (const Params& p, const Frame& f, const NodePos& n, unsigned long long& upd, unsigned long long& vis)
-{
-  Counters cnt; cnt.n_updates = 0; cnt.n_visits = 0;
-  int rc = update_voxel_dfs (p, f, n, cnt);
-  upd += cnt.n_updates; vis += cnt.n_visits - 1;
-  if (p.diag) { atomicAdd (&p.diag[0], 1ull); atomicAdd (&p.diag[1], (unsigned long long) cnt.n_visits); }
-  return rc;
-}
 // leaf visit (hpp:143-218) of a node whose pre-existing children were just pruned, by one WARP: if the node
 // re-splits, its eight fresh children are visited by lanes 0..7 in parallel (their subtrees are disjoint).
 // All 32 lanes must call it with the same node.  Returns the node's return code in every lane.

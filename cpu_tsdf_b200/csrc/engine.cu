@@ -221,9 +221,14 @@ __global__ void k_front (Params p, const FrameRec* __restrict__ fr, int cull_blo
   if (split_it) presplit_point (p, fx_, fy_, fz_);
 }
 
-// general path: one thread per culled coarse cell runs updateVoxel depth-first
-__global__ void k_update_dfs (Params p, Frame f, const int* __restrict__ list, const int* __restrict__ count, unsigned long long* __restrict__ stats)
+// general path: one thread per culled coarse cell runs updateVoxel depth-first.  The frame and its counter set come from
+// the record, like the other kernels of a frame, so the launch can be captured and replayed.
+__global__ void k_update_dfs (Params p, const FrameRec* __restrict__ fr, const int* __restrict__ list, const int* __restrict__ d_count,
+                              unsigned long long* __restrict__ stats)
 {
+  const int* count = d_count + 16 * fr->cset;
+  if ((int) (blockIdx.x * blockDim.x) >= *count) return;  // (whole block: the grid covers every coarse cell)
+  B2_SHARED_FRAME (fr)
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= *count) return;
   int n = 1 << p.C;
@@ -601,7 +606,7 @@ struct b200tsdf
   unsigned char* d_frame[2] = { nullptr, nullptr };
   size_t frame_cap = 0;
   cudaEvent_t ev_copied[2] = { nullptr, nullptr }, ev_consumed[2] = { nullptr, nullptr };
-  cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr, ev_k0 = nullptr, ev_k1 = nullptr;
+  cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
   uint64_t frame_no = 0;
   int count_set = 0;             // which of the two per-frame counter sets the last frame used
   int* d_culled = nullptr; int* d_count = nullptr; unsigned long long* d_stats = nullptr;
@@ -612,15 +617,13 @@ struct b200tsdf
   bool is_empty = true;          // TSDFVolumeOctree::is_empty_ (cpp:205, hpp:101)
   // fast-path work queues (levels C .. L-3)
   Queues Q{}; int q_levels = 0; QNode* q_mem = nullptr; size_t q_mem_cap = 0;
-  int* d_blist = nullptr; int* d_bail = nullptr; size_t blist_cap = 0;
+  int* d_blist = nullptr; size_t blist_cap = 0;
   // fused per-cell upper sweeps (coarse cells are the top-tier roots and the block roots are <= 3 levels below)
   // supercell path: sl = level of the tier-1 roots, nup = coarse levels above them (swept by k_upper_*), super_static = number of
-  // supercells when every tier-1 root is one (coarse cells inside the brick), replayable = the frame's launches read only the record
+  // supercells when every tier-1 root is one (coarse cells inside the brick)
   int cell_cap = 0; QNode* d_cellq = nullptr; size_t cellq_cap = 0; CellTop* d_celltop = nullptr; QNode* d_superq = nullptr;
-  bool top_path = false, replayable = false; int sl = 0, nup = 0, super_static = 0;
+  bool top_path = false; int sl = 0, nup = 0, super_static = 0;
   bool fast_path = false; int force_general = 0;
-  bool use_pdl = true;           // programmatic dependent launch between the hot kernels (B200TSDF_PDL=0 turns it off)
-  int bd_minb = 6;               // resident CTAs per SM the brick kernel is compiled for (80 registers; tuning knob: B200TSDF_BD_MINB=6|8)
   // device copy of Params (the rare out-of-line paths read it through a pointer) and the ring of per-frame records
   Params* d_params = nullptr;
   unsigned long long* d_dbg = nullptr;     // phase-timing counters of k_celltop_up once b200tsdf_debug_timing armed them
@@ -633,7 +636,7 @@ struct b200tsdf
   // robin — the host only waits when it is BATCH_SEGS batches ahead of the device
   FrameRec* d_bring = nullptr; FrameRec* h_bring = nullptr; int bring_half = 0; int bring_seg = 0; bool bring_used[BATCH_SEGS] = {};
   cudaEvent_t ev_bring[BATCH_SEGS] = {};
-  cudaEvent_t ev_half_done[2] = { nullptr, nullptr }; bool half_used[2] = { false, false }; FrameRec* batch_recs = nullptr;
+  cudaEvent_t ev_half_done[2] = { nullptr, nullptr }; bool half_used[2] = { false, false };
   cudaGraphExec_t batch_exec[2][FRAME_RING / 2 + 1] = {};
   // multi-GPU (multigpu.cuh): NCCL communicator (opaque here), row-sliced uploads
   void* comm = nullptr; int comm_rank = 0, comm_size = 1;
@@ -840,11 +843,9 @@ int b200tsdf_create (const b200tsdf_config* cfg, b200tsdf_t** out)
   b200tsdf* h = new b200tsdf;
   if (cfg) h->cfg_pending = *cfg; else b200tsdf_default_config (&h->cfg_pending);
   h->device = h->cfg_pending.device;
-  if (const char* e = std::getenv ("B200TSDF_PDL")) h->use_pdl = std::atoi (e) != 0;
   if (const char* e = std::getenv ("B200TSDF_ROWS_CHUNK")) { const int v = std::atoi (e); if (v >= 1 && v <= 32) h->rows_chunk = v; }
   if (const char* e = std::getenv ("B200TSDF_HOST_PACK")) h->host_pack = std::atoi (e) != 0 ? 1 : 0;
   if (const char* e = std::getenv ("B200TSDF_PACK_THREADS")) { const int v = std::atoi (e); if (v >= 1 && v <= 256) h->pack_threads = v; }
-  if (const char* e = std::getenv ("B200TSDF_BD_MINB")) { const int v = std::atoi (e); if (v == 6 || v == 8) h->bd_minb = v; }
   if (h->device < 0 || h->device >= ndev) { delete h; return B200TSDF_EINVAL; }
   bool ok = cudaSetDevice (h->device) == cudaSuccess
          && cudaDeviceGetAttribute (&h->sm_count, cudaDevAttrMultiProcessorCount, h->device) == cudaSuccess
@@ -870,7 +871,6 @@ int b200tsdf_create (const b200tsdf_config* cfg, b200tsdf_t** out)
     ok = cudaEventCreateWithFlags (&h->ev_copied[i], cudaEventDisableTiming) == cudaSuccess
       && cudaEventCreateWithFlags (&h->ev_consumed[i], cudaEventDisableTiming) == cudaSuccess;
   ok = ok && cudaEventCreate (&h->ev_t0) == cudaSuccess && cudaEventCreate (&h->ev_t1) == cudaSuccess
-          && cudaEventCreate (&h->ev_k0) == cudaSuccess && cudaEventCreate (&h->ev_k1) == cudaSuccess
           && cudaEventCreate (&h->ev_p0) == cudaSuccess && cudaEventCreate (&h->ev_p1) == cudaSuccess;
   for (int i = 0; ok && i < 64; ++i) ok = cudaEventCreateWithFlags (&h->ev_rows_ready[i / 32][i % 32], cudaEventDisableTiming) == cudaSuccess
                                           && cudaEventCreateWithFlags (&h->ev_rows_up[i / 32][i % 32], cudaEventDisableTiming) == cudaSuccess;
@@ -912,10 +912,9 @@ void b200tsdf_destroy (b200tsdf_t* h)
   for (int i = 0; i < RENDER_SEGS; ++i) if (h->ev_rrec[i]) cudaEventDestroy (h->ev_rrec[i]);
   for (int i = 0; i < BATCH_SEGS; ++i) if (h->ev_bring[i]) cudaEventDestroy (h->ev_bring[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_half_done[i]) cudaEventDestroy (h->ev_half_done[i]);
-  cudaFree (h->d_frame[0]); cudaFree (h->d_frame[1]); cudaFree (h->q_mem); cudaFree (h->d_blist); cudaFree (h->d_bail); cudaFree (h->d_cellq); cudaFree (h->d_superq); cudaFree (h->d_celltop);
+  cudaFree (h->d_frame[0]); cudaFree (h->d_frame[1]); cudaFree (h->q_mem); cudaFree (h->d_blist); cudaFree (h->d_cellq); cudaFree (h->d_superq); cudaFree (h->d_celltop);
   for (int i = 0; i < 2; ++i) { if (h->ev_copied[i]) cudaEventDestroy (h->ev_copied[i]); if (h->ev_consumed[i]) cudaEventDestroy (h->ev_consumed[i]); }
   if (h->ev_t0) cudaEventDestroy (h->ev_t0); if (h->ev_t1) cudaEventDestroy (h->ev_t1);
-  if (h->ev_k0) cudaEventDestroy (h->ev_k0); if (h->ev_k1) cudaEventDestroy (h->ev_k1);
   if (h->ev_p0) cudaEventDestroy (h->ev_p0); if (h->ev_p1) cudaEventDestroy (h->ev_p1);
   for (int i = 0; i < KRING; ++i) { if (h->kring[i][0]) cudaEventDestroy (h->kring[i][0]); if (h->kring[i][1]) cudaEventDestroy (h->kring[i][1]); }
   if (h->stream) cudaStreamDestroy (h->stream);
@@ -1026,7 +1025,7 @@ int b200tsdf_reset (b200tsdf_t* h)
     h->sl = np.L - 6;
     h->nup = std::max (0, h->sl - np.C);
     h->super_static = 0;
-    h->top_path = h->fast_path && np.T >= 2 && h->sl >= 0 && !(c.debug_flags & 6);
+    h->top_path = h->fast_path && np.T >= 2 && h->sl >= 0 && !(c.debug_flags & 2);
     if (h->top_path && np.C > h->sl)
     {
       // every tier-1 root is a supercell; they must be the root-array nodes (T == 2) and fit the per-cell scratch
@@ -1046,14 +1045,12 @@ int b200tsdf_reset (b200tsdf_t* h)
       }
       if (h->super_static && !h->d_superq) CK (cudaMalloc (&h->d_superq, 4096 * sizeof (QNode)));
     }
-    h->replayable = h->fast_path;                         // every kernel of the brick paths reads the frame from its record (the general depth-first kernel takes it by value)
     size_t bl = h->q_levels ? caps[h->q_levels - 1] : 0;
     if (h->top_path) bl = std::max (bl, (size_t) h->cell_cap * 512);
     if (bl > h->blist_cap)
     {
-      cudaFree (h->d_blist); cudaFree (h->d_bail); h->d_blist = h->d_bail = nullptr; h->blist_cap = 0;
+      cudaFree (h->d_blist); h->d_blist = nullptr; h->blist_cap = 0;
       CK (cudaMalloc (&h->d_blist, bl * BL_CLASSES * sizeof (int)));          // one list per work class
-      CK (cudaMalloc (&h->d_bail, bl * sizeof (int)));
       h->blist_cap = bl;
     }
   }
@@ -1069,7 +1066,6 @@ int b200tsdf_reset (b200tsdf_t* h)
   }
   p.err = h->d_err;
   p.pix = h->d_pix;
-  p.diag = h->d_stats + 3;
   p.dbg = h->d_dbg;
   CK (cudaMemcpyAsync (h->d_params, &p, sizeof (Params), cudaMemcpyHostToDevice, h->stream));
   CK (cudaStreamSynchronize (h->stream));                            // (&p is host memory that may change after reset)
@@ -1117,20 +1113,16 @@ static void fill_rec (b200tsdf* h, FrameRec& r, const unsigned char* d_pts, size
   r.pad_[0] = r.pad_[1] = 0; r.kt[0] = r.kt[1] = 0;
 }
 
-// the launches of one frame.  `rec` is the host image of *d_rec (only the paths that are not replayable read it).
+// the launches of one frame; every kernel reads the frame from *d_rec, so the launches can be captured and replayed.
 // with_events: bracket the dominant kernel with an event pair of the ring (never inside a capture)
-static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec& rec, const FrameRec* d_rec, bool with_events)
+static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, bool with_events)
 {
   const Params& p = h->p;
-  const Frame& f = rec.f;
-  int* cnt = h->d_count + 16 * rec.cset;
-  const int npix = f.width * f.height;
+  const int npix = h->cfg.image_width * h->cfg.image_height;   // (every frame has this size: check_cloud_layout)
   const int ncells = 1 << (3 * p.C);
   {
     const int cull_blocks = (ncells + 255) / 256;
-    const bool pdl = h->replayable && h->use_pdl;
-    if (pdl) CK (launch_pdl (k_front, dim3 (cull_blocks + (npix + 255) / 256), dim3 (256), s, p, d_rec, cull_blocks, h->d_culled, h->d_count, h->Q.q[0], h->d_stats));
-    else k_front<<<cull_blocks + (npix + 255) / 256, 256, 0, s>>> (p, d_rec, cull_blocks, h->d_culled, h->d_count, h->fast_path ? h->Q.q[0] : nullptr, h->d_stats);
+    CK (launch_pdl (k_front, dim3 (cull_blocks + (npix + 255) / 256), dim3 (256), s, p, d_rec, cull_blocks, h->d_culled, h->d_count, h->Q.q[0], h->d_stats));
   }
   h->launches += 1;
   int kr = -1;
@@ -1150,8 +1142,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec& rec, const
       QNode* cells = h->super_static ? h->d_superq : h->Q.q[h->nup];
       const int qslot = h->super_static ? -1 : h->nup;
       auto kd = p.color ? k_celltop_down<true> : k_celltop_down<false>;
-      if (h->use_pdl) CK (launch_pdl (kd, dim3 (h->sm_count * 4), dim3 (TOP_THREADS), s, p, d_rec, cells, h->d_count, h->d_cellq, h->d_celltop, h->cell_cap, h->d_blist, (int) h->blist_cap, h->d_stats, h->sl, qslot, h->super_static));
-      else kd<<<h->sm_count * 4, TOP_THREADS, 0, s>>> (p, d_rec, cells, h->d_count, h->d_cellq, h->d_celltop, h->cell_cap, h->d_blist, (int) h->blist_cap, h->d_stats, h->sl, qslot, h->super_static);
+      CK (launch_pdl (kd, dim3 (h->sm_count * 4), dim3 (TOP_THREADS), s, p, d_rec, cells, h->d_count, h->d_cellq, h->d_celltop, h->cell_cap, h->d_blist, (int) h->blist_cap, h->d_stats, h->sl, qslot, h->super_static));
       h->launches++;
       bq = h->d_cellq;
     }
@@ -1163,9 +1154,9 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec& rec, const
     if (kr >= 0) CK (cudaEventRecord (h->kring[kr][0], s));
     // the dominant kernel: one warp per interior block root, the brick updated in place
     {
-      auto kb = h->bd_minb == 6 ? (p.color ? k_bricks<true, 6> : k_bricks<false, 6>) : (p.color ? k_bricks<true, 8> : k_bricks<false, 8>);
-      const dim3 g (h->sm_count * h->bd_minb), b (BD_WARPS * 32);
-      if (h->top_path && h->use_pdl) CK (launch_pdl (kb, g, b, s, p, (const Params*) h->d_params, d_rec, bq, (const int*) h->d_blist, (int) h->blist_cap, h->d_count, h->d_stats, p.L - 3));
+      auto kb = p.color ? k_bricks<true> : k_bricks<false>;
+      const dim3 g (h->sm_count * BD_CTAS), b (BD_WARPS * 32);
+      if (h->top_path) CK (launch_pdl (kb, g, b, s, p, (const Params*) h->d_params, d_rec, bq, (const int*) h->d_blist, (int) h->blist_cap, h->d_count, h->d_stats, p.L - 3));
       else kb<<<g, b, 0, s>>> (p, h->d_params, d_rec, bq, h->d_blist, (int) h->blist_cap, h->d_count, h->d_stats, p.L - 3);
     }
     if (kr >= 0) CK (cudaEventRecord (h->kring[kr][1], s));
@@ -1175,8 +1166,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec& rec, const
       QNode* cells = h->super_static ? h->d_superq : h->Q.q[h->nup];
       const int qslot = h->super_static ? -1 : h->nup;
       auto ku = p.color ? k_celltop_up<true> : k_celltop_up<false>;
-      if (h->use_pdl) CK (launch_pdl (ku, dim3 (h->sm_count), dim3 (128), s, p, d_rec, cells, (const int*) h->d_count, (const QNode*) h->d_cellq, (const CellTop*) h->d_celltop, h->cell_cap, h->d_stats, h->sl, qslot, h->super_static));
-      else ku<<<h->sm_count, 128, 0, s>>> (p, d_rec, cells, h->d_count, h->d_cellq, h->d_celltop, h->cell_cap, h->d_stats, h->sl, qslot, h->super_static);
+      CK (launch_pdl (ku, dim3 (h->sm_count), dim3 (128), s, p, d_rec, cells, (const int*) h->d_count, (const QNode*) h->d_cellq, (const CellTop*) h->d_celltop, h->cell_cap, h->d_stats, h->sl, qslot, h->super_static));
       h->launches++;
       for (int li = h->nup - 1; li >= 0; --li) { k_upper_up<<<h->sm_count * 2, 128, 0, s>>> (p, d_rec, h->Q, li, h->d_stats); h->launches++; }
     }
@@ -1187,7 +1177,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec& rec, const
   {
     if (kr >= 0) CK (cudaEventRecord (h->kring[kr][0], s));
     // general path: every culled cell depth-first (grid covers the worst case; threads past *count exit)
-    k_update_dfs<<<(ncells + 31) / 32, 32, 0, s>>> (p, f, h->d_culled, cnt, h->d_stats);
+    k_update_dfs<<<(ncells + 31) / 32, 32, 0, s>>> (p, d_rec, h->d_culled, h->d_count, h->d_stats);
     if (kr >= 0) CK (cudaEventRecord (h->kring[kr][1], s));
     h->launches++;
   }
@@ -1223,7 +1213,7 @@ static int integrate_on_device (b200tsdf* h, const unsigned char* d_pts, size_t 
   fill_rec (h, rec, d_pts, stride, xyz_off, rgba_off, W, H, pose);
   if (h->time_frames) CK (cudaEventRecord (h->ev_t0, s));
   CK (cudaMemcpyAsync (h->d_ring + slot, &rec, sizeof (FrameRec), cudaMemcpyHostToDevice, s));
-  { int rc = launch_frame (h, s, rec, h->d_ring + slot, h->time_frames); if (rc) return rc; }
+  { int rc = launch_frame (h, s, h->d_ring + slot, h->time_frames); if (rc) return rc; }
   if (h->time_frames) CK (cudaEventRecord (h->ev_t1, s));
   note_device_err (h, s);
   { int rc = ring_advance (h, slot, s); if (rc) return rc; }
@@ -1278,7 +1268,6 @@ static int batch_records (b200tsdf* h, int m, const void* const* d_points, size_
   CK (cudaMemcpyAsync (h->d_bring + a * HALF, recs, (size_t) m * sizeof (FrameRec), cudaMemcpyHostToDevice, rec_stream));
   CK (cudaEventRecord (h->ev_bring[sg], rec_stream));      // the staging segment is free again once this copy has run
   h->bring_used[sg] = true; h->bring_seg = (sg + 1) % BATCH_SEGS;
-  h->batch_recs = recs;
   return B200TSDF_OK;
 }
 static int batch_launch (b200tsdf* h, int m)
@@ -1293,7 +1282,7 @@ static int batch_launch (b200tsdf* h, int m)
     cudaGraph_t g = nullptr;
     CK (cudaStreamBeginCapture (s, cudaStreamCaptureModeThreadLocal));
     int rc = B200TSDF_OK;
-    for (int i = 0; i < m && rc == B200TSDF_OK; ++i) rc = launch_frame (h, s, h->batch_recs[i], h->d_bring + a * HALF + i, false);
+    for (int i = 0; i < m && rc == B200TSDF_OK; ++i) rc = launch_frame (h, s, h->d_bring + a * HALF + i, false);
     cudaError_t ce = cudaStreamEndCapture (s, &g);
     h->launches_per_frame = (int) ((h->launches - l0) / std::max (1, m));
     h->launches = l0; h->prof_frames = f0;
@@ -1327,14 +1316,6 @@ int b200tsdf_integrate_batch_device (b200tsdf_t* h, int n, const void* const* d_
   for (int done = 0; done < n;)
   {
     const int m = std::min (HALF, n - done);
-    if (!h->replayable)
-    {
-      // the general depth-first kernel takes the frame by value: frame by frame
-      for (int i = 0; i < m; ++i)
-        if (int rc = integrate_on_device (h, (const unsigned char*) d_points[done + i], stride, xyz_off, rgba_off, width, height, poses_c2w + 16 * (size_t) (done + i))) return rc;
-      done += m;
-      continue;
-    }
     if (int rc = batch_records (h, m, d_points + done, stride, xyz_off, rgba_off, width, height, poses_c2w + 16 * (size_t) done, h->stream)) return rc;
     if (int rc = batch_launch (h, m)) return rc;
     done += m;
@@ -1552,8 +1533,7 @@ int b200tsdf_get_stats (b200tsdf_t* h, b200tsdf_stats* s)
   s->n_updates = (int64_t) (st[ST_UPDATES] - st[ST_N + ST_UPDATES]);
   s->n_node_visits = (int64_t) (st[ST_VISITS] - st[ST_N + ST_VISITS]);
   s->n_block_visits = (int64_t) (st[ST_BLOCKS] - st[ST_N + ST_BLOCKS]);
-  s->reserved = (int32_t) (st[3] - st[ST_N + 3]);          // diagnostics: slow folds in the last frame
-  s->n_bail = cnt[10]; s->n_slow_visits = (int64_t) (st[4] - st[ST_N + 4]);
+  s->reserved = 0; s->n_bail = 0; s->n_slow_visits = 0;   // (kept for the layout; always 0)
   s->n_culled_cells = cnt[0];
   s->pool_capacity = (int64_t) h->pool;
   s->coarse_level = h->p.C; s->finest_level = h->p.L; s->tiers = h->p.T;

@@ -197,8 +197,7 @@ int b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows
   if (hpack) ensure_pack_pool (h, nr);
   // three-stage pipeline over chunks of frames: the copy stream only uploads (the copy engine never waits for a kernel), the
   // gather stream packs and all-gathers, the compute stream fuses.  Chunks are ROWS_CHUNK frames, the last one is halved down
-  // to 2 so that little is left to upload and fuse once the last pixel has been packed.  Configurations without replayable
-  // launches are fused frame by frame once their chunk has arrived.
+  // to 2 so that little is left to upload and fuse once the last pixel has been packed.
   cudaStream_t cs = h->copy_stream, gs = h->gather_stream;
   if (int rc = pending_device_err (h)) return rc;
   if (h->rows_used[s]) { CK (cudaStreamWaitEvent (cs, h->ev_rows_done[s], 0)); CK (cudaStreamWaitEvent (gs, h->ev_rows_done[s], 0)); }
@@ -255,7 +254,7 @@ int b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows
         if (!h->pack_pool->help ()) std::this_thread::yield ();
     if (trace) { const double t = now (); t_pack += t - t0; t0 = t; }
     // the chunk's frame records travel on the copy stream ahead of its frames
-    if (h->replayable) { if (int rc = batch_records (h, m, ptrs, f_stride, f_xyz, f_rgba, width, height, poses_c2w + 16 * (size_t) c0, cs)) return rc; }
+    if (int rc = batch_records (h, m, ptrs, f_stride, f_xyz, f_rgba, width, height, poses_c2w + 16 * (size_t) c0, cs)) return rc;
     if (hpack)
     {
       if (npts)
@@ -298,10 +297,7 @@ int b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows
       CK (cudaEventRecord (ready, gs));
     }
     CK (cudaStreamWaitEvent (h->stream, ready, 0));
-    if (h->replayable) { if (int rc = batch_launch (h, m)) return rc; }
-    else
-      for (int i = 0; i < m; ++i)
-        if (int rc = integrate_on_device (h, (const unsigned char*) ptrs[i], f_stride, f_xyz, f_rgba, width, height, poses_c2w + 16 * (size_t) (c0 + i))) return rc;
+    if (int rc = batch_launch (h, m)) return rc;
     if (trace) t_enq += now () - t0;
   }
   CK (cudaEventRecord (h->ev_rows_done[s], h->stream));

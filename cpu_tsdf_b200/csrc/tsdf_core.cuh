@@ -163,7 +163,6 @@ struct Params
   int* root_ns;
   unsigned char* work;        // [pool] finest-tier bricks: interior level-2 nodes seen by the last update (scheduling hint only)
   int* err;                   // device error bits
-  unsigned long long* diag;   // [0] slow folds in the upper sweeps, [1] visits inside them (this handle's counters; may be null)
   unsigned long long* dbg;    // optional phase timing of k_celltop_up (b200tsdf_debug_timing), normally null
   uint32_t* pix;              // [width * height] pixel plane of the current frame, written by k_front: {z bits, bgra} per pixel
                               // with colour, z bits alone without (read by the fast observation, obs_fast.cuh)

@@ -54,7 +54,7 @@ typedef struct b200tsdf_config
   int32_t device;                           /* CUDA device ordinal                                */
   int32_t pool_log2;                        /* brick pool capacity = 2^pool_log2 (0 = default 20) */
   int32_t shard_rank, shard_count;          /* this handle owns coarse cells with hash(cell) % shard_count == shard_rank */
-  int32_t debug_flags;                      /* bit0: general depth-first update kernel only; bit1: per-level upper sweeps instead of the fused per-cell ones; bit2: generic per-cell sweeps instead of the speculative tier-1 ones */
+  int32_t debug_flags;                      /* bit0: general depth-first update kernel only; bit1: per-level upper sweeps instead of the fused per-cell ones; other bits are ignored */
   int32_t color_mode;                       /* setColorMode (tsdf_volume_octree.h:290) — B200TSDF_COLOR_RGB (default) or B200TSDF_COLOR_RGB_NORMALIZED
                                                (octree.cpp:379-434; fused by the general kernel).  "LAB" (octree.cpp:436-581) is refused: RGB2LAB needs libm pow */
   int32_t reserved[2];
@@ -94,8 +94,8 @@ int  b200tsdf_integrate_device (b200tsdf_t* h, const void* d_points, size_t stri
  * parameters go to the device in one copy and the launches of the whole batch are one CUDA-graph launch (captured once
  * per batch size, replayed afterwards), so the host issues ~3 driver calls per batch instead of ~6 per frame.
  * d_points: n device pointers (same layout for all); poses_c2w: n row-major 4x4 matrices back to back.  Asynchronous
- * like b200tsdf_integrate_device.  Configurations fused by the general depth-first kernel (track_variance, RGBNormalized payload)
- * are fused frame by frame inside the same call. */
+ * like b200tsdf_integrate_device.  Every configuration takes this path, those fused by the general depth-first kernel
+ * (track_variance, RGBNormalized payload) included. */
 int  b200tsdf_integrate_batch_device (b200tsdf_t* h, int n, const void* const* d_points, size_t stride, int xyz_off, int rgba_off,
                                       int width, int height, const double* poses_c2w);
 /* streaming variant of b200tsdf_integrate for producers that keep their (pinned) frame buffers alive:
@@ -264,11 +264,11 @@ typedef struct b200tsdf_stats
   int64_t n_bricks;         /* allocated bricks */
   int64_t n_block_visits;   /* finest-tier bricks processed in the last frame */
   int64_t pool_capacity;
-  int32_t coarse_level, finest_level, tiers, reserved;   /* reserved: upper-level slow folds in the last frame */
+  int32_t coarse_level, finest_level, tiers, reserved;   /* reserved: always 0 */
   double  ms_last_integrate;   /* device time of the last integrate (CUDA events on the handle's stream) */
   double  ms_last_kernel;      /* device time of the dominant (brick update) kernel in the last integrate */
-  int64_t n_bail;              /* block roots handed to the general path in the last frame (prune-then-resplit) */
-  int64_t n_slow_visits;       /* node visits made by the general path inside the upper sweeps in the last frame */
+  int64_t n_bail;              /* always 0 (kept for the layout) */
+  int64_t n_slow_visits;       /* always 0 (kept for the layout) */
 } b200tsdf_stats;
 int  b200tsdf_get_stats (b200tsdf_t* h, b200tsdf_stats* s);
 

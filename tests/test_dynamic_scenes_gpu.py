@@ -3,8 +3,8 @@ pruned and nodes re-split in the same call.
 
 * Parity: every case, bit for bit against the restatement and against the reference build's digests
   (tests/golden/dynamic_pins.json), through the route reset() picks, the general depth-first kernel (debug_flags bit 0),
-  the per-level upper sweeps (bit 1), the generic per-cell sweeps (bit 2), and for K1 and K4 integrateBatchDevice in
-  graph-replayed batches.  The per-frame routes compare addObservation counts frame by frame.
+  the per-level upper sweeps (bit 1), and for K1 to K5 integrateBatchDevice in graph-replayed batches (K1, K4 and K5
+  also with the general kernel).  The per-frame routes compare addObservation counts frame by frame.
 * Coverage on the device: the diagnostic counters of k_celltop_up show that the slow paths these streams exist for ran.
 * The fresh invariant on raw storage: after every frame of the carve phase, every node that does not exist, in every
   claimed brick, is exactly in the constructor state.
@@ -27,7 +27,7 @@ def pool_log2(case):
     return {256: 17, 512: 18, 2048: 18, 4096: 19}[case.res]
 
 
-BATCH = 2                                          # frames per integrateBatchDevice call (K1 and K4 have 10 frames)
+BATCH = 2                                          # frames per integrateBatchDevice call (every batched case has an even number)
 
 
 class EngineAdapter:
@@ -87,17 +87,21 @@ def differing(got, want):
     return [k for k in want if got.get(k) != want[k]] + [k for k in got if k not in want]
 
 
-FLAGS = {"reset": 0, "general": 1, "upper": 2, "generic": 4}
-ROUTES = [(cid, r) for r in FLAGS for cid in IDS] + [("K1", "batch"), ("K4", "batch")]
+FLAGS = {"reset": 0, "general": 1, "upper": 2}
+BATCHED = {"batch": 0, "general_batch": 1}         # integrateBatchDevice on the route reset() picks / the general kernel
+# K2 (variance) and K3 (RGBNormalized) take the general kernel, and general_batch forces it on brick-route shapes: their
+# batches are graph launches as well.  K6 pins its nodes after every one of its 9 frames, so it is not fused in pairs.
+ROUTES = [(cid, r) for r in FLAGS for cid in IDS] + [(cid, "batch") for cid in ("K1", "K2", "K3", "K4", "K5")] \
+    + [(cid, "general_batch") for cid in ("K1", "K4", "K5")]
 
 
 @pytest.mark.parametrize("cid,route", ROUTES)
 def test_engine_matches_restatement(cid, route):
     case = CASES[cid]
-    e = EngineAdapter(case, flags=FLAGS.get(route, 0), batch=route == "batch")
+    e = EngineAdapter(case, flags={**FLAGS, **BATCHED}[route], batch=route in BATCHED)
     got = digests(outputs(case, e))
     want = port_digests(cid)
-    if route == "batch":                       # one count per batch: the last frame's
+    if route in BATCHED:                       # one count per batch: the last frame's
         want = {k: v for k, v in want.items() if k != "n_updates"}
         assert e.v.profile_end().graph_launches == len(case.poses) // BATCH
     assert differing(got, want) == []
@@ -120,8 +124,8 @@ _coverage = {}
 
 
 def coverage(cid):
-    """per stream, on a handle of its own: the sums of debug counters [6..10], of stats.reserved (slow folds of the upper
-    sweeps), n_slow_visits and n_bail"""
+    """per stream, on a handle of its own: the sums of debug counters [6..10], of stats.reserved, n_slow_visits and n_bail
+    (the last three are always 0)"""
     if cid not in _coverage:
         case = CASES[cid]
         e = EngineAdapter(case)
@@ -167,8 +171,7 @@ def coarse_prunes(vol, case):
 def test_upper_sweeps_fold_a_carved_region():
     """K5 (4096^3 / 10 m) has a coarse level above the supercells, which only k_upper_down / k_upper_up sweep on the route
     reset() picks.  Coarse nodes whose children were all pruned must lose their split flag in the same frames as in the
-    restatement, and some must.  (stats.reserved and n_slow_visits cannot show this: they read Params::diag, which only
-    upper_fold_slow writes, and nothing calls it, so both are zero on every stream.)"""
+    restatement, and some must.  (stats.reserved and n_slow_visits cannot show this: they are always 0.)"""
     case = CASES["K5"]
     dev = coarse_prunes(EngineAdapter(case), case)
     ref = coarse_prunes(OracleAdapter(case), case)
@@ -179,9 +182,8 @@ def test_upper_sweeps_fold_a_carved_region():
 
 
 def test_bail_counter_is_never_written():
-    """stats.n_bail reads per-frame counter slot 10, and no kernel writes that slot any more (slot 0: culled cells, 1-8:
-    queue levels, 9 and 12-14: the brick lists, 11: the brick work cursor; the slot is only cleared), so it is zero on every
-    stream.  If a kernel starts writing it again, this test fails and should become a real assertion."""
+    """stats.n_bail is always 0 (no kernel hands block roots to a bail-out list: the prune-then-resplit case is visited in
+    place), on every stream.  If it is ever given a meaning again, this test fails and should become a real assertion."""
     for cid in IDS:
         assert coverage(cid)["bail"] == 0
 
