@@ -12,6 +12,8 @@
 namespace b2 {
 
 inline int ilog2_exact (int v) { int l = 0; while ((1 << l) < v && l < 30) ++l; return ((1 << l) == v) ? l : -1; }
+// the smallest float not below t: for every float d, d < at_least (t) <=> (double) d < t (the host twin of float_at_least)
+inline float at_least (double t) { float f = (float) t; if ((double) f < t) f = std::nextafterf (f, INFINITY); return f; }
 
 // returns nullptr on success or a message describing the unsupported configuration
 inline const char* derive_params (const b200tsdf_config& c, Params& p, size_t& pool, size_t& root_n)
@@ -48,7 +50,6 @@ inline const char* derive_params (const b200tsdf_config& c, Params& p, size_t& p
   p.fx_f = (float) c.fx; p.fy_f = (float) c.fy; p.cx_f = (float) c.cx; p.cy_f = (float) c.cy;
   p.fast_proj = (c.image_width < 8192 && c.image_height < 8192 && std::fabs (c.cx) < 1e4 && std::fabs (c.cy) < 1e4) ? 1 : 0;
   {
-    auto at_least = [] (double t) { float f = (float) t; if ((double) f < t) f = std::nextafterf (f, INFINITY); return f; };
     p.rc_lo_f = at_least (-0.99); p.rc_hi_f = at_least (p.rc_thresh);
     // error of the float pixel estimate a = x*fx*rcp(z) + cx against the reference's double expression: the product
     // and the approximate reciprocal contribute < 2^-22 |x fx / z|, the final rounding 2^-24 |a| (brick_direct.cuh)
@@ -57,9 +58,11 @@ inline const char* derive_params (const b200tsdf_config& c, Params& p, size_t& p
     if (!(p.proj_guard < 0.05f)) p.fast_proj = 0;
     // the operands of the brick kernels' divisions (div_with): d_new, clamped to [-max_dist_neg, max_dist_pos], over
     // max_dist_neg; the weighted sums over w + 1 <= max_weight + 1.  The sensor bounds are not among them, so the
-    // integrate program's default min_sensor_dist = 0 keeps the brick kernels.
+    // integrate program's default min_sensor_dist = 0 keeps the brick kernels (div_with sends a tiny distance numerator to
+    // the IEEE division).  A weight cap of 0 or >= 1e-20 keeps the colour numerators w c + c', divided by div_fast alone,
+    // at 0 or >= 1e-20, far inside the region where div_fast is exact (obs_fast.cuh).
     p.exact_div_ok = (c.max_dist_neg >= 1e-6f && c.max_dist_neg <= 1e6f && std::fabs (c.max_dist_pos) <= 1e6f
-                      && c.max_weight >= 0.f && c.max_weight <= 1e9f) ? 1 : 0;
+                      && (c.max_weight == 0.f || c.max_weight >= 1e-20f) && c.max_weight <= 1e9f) ? 1 : 0;
   }
   p.color = c.integrate_color != 0; p.track_var = c.track_variance != 0;
   if (c.color_mode == B200TSDF_COLOR_LAB)

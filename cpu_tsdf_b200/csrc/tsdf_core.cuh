@@ -479,14 +479,16 @@ struct Obs
 
 // reprojectPoint (tsdf_volume_octree.cpp:611-617): u = (int)(x*fx/z + cx) in DOUBLE, truncation toward
 // zero.  The double divide is ~10x the cost of everything else in a node visit, so a float estimate
-// is tried first and accepted only where it provably truncates to the same integer: its error is
-// below 2^-24 * (3.01|x fx/z| + |cx| + |a|) < 4e-3 for |a| < 3e4, and the estimate must sit at least
+// is tried first and accepted only where it truncates to the same integer: its error is below
+// 2^-24 * (3.01|x fx/z| + |cx| + |a|), about 7.2e-3 at cx = 320 and 9.6e-3 at |cx| near 1e4 for |a| < 3e4
+// (measured on the H100: at most 4.2e-3, tests/test_fast_arith_gpu.py), and the estimate must sit at least
 // 1e-2 away from an integer (and above 0).  Otherwise the reference's double expression is evaluated.
+B2_HD float project1_estimate (float x, float z, float ff, float cf) { return fadd (fdiv (fmul (x, ff), z), cf); }
 B2_HD int project1 (const Params& p, float x, float z, double fd, double cd, float ff, float cf)
 {
   if (p.fast_proj)
   {
-    float a = fadd (fdiv (fmul (x, ff), z), cf);
+    float a = project1_estimate (x, z, ff, cf);
     float fr = a - floorf (a);
     if (a > 0.01f && a < 30000.f && fr > 0.01f && fr < 0.99f) return (int) a;
   }

@@ -102,7 +102,19 @@ class Case:
                 yield pose, cloud
 
 
+def near_node_pose(pose, size, level, depth=4e-4, side=(3e-5, -2e-5)):
+    """`pose` moved so that the nearest centre of a node at `level` (grid edge `size`) lies `depth` metres in front of the
+    camera along its viewing axis and `side` metres off it (x, y of the camera frame): that node is seen at a fraction of a
+    millimetre of depth, well inside the image"""
+    h = size / 2 ** level
+    c = (np.floor((pose[:3, 3] + size / 2) / h) + 0.5) * h - size / 2
+    out = pose.copy()
+    out[:3, 3] = c - depth * pose[:3, 2] - side[0] * pose[:3, 0] - side[1] * pose[:3, 1]
+    return out
+
+
 S1, S2 = synth.S1, synth.S2
+STRIP = synth.Camera(4096.0, 128.0, 4095.5, 31.5, 8191, 64)              # the widest image with the float projection on
 ROOM1 = synth.Scene(room_half=1.0, cam_radius=0.5, sphere=False)          # walls on node boundaries of a 4 m grid
 
 
@@ -133,6 +145,19 @@ def _cases():
     # outside the range where the brick kernels' division is exact: the weighted sum overflows to inf and is then divided
     cs.append(Case("D1", 512, 3.0, synth.Camera(525.0, 525.0, 320.0, 240.0), S1, random_poses(S1, 1, 108), repeat=10,
                    params=dict(max_dist_pos=10.0, max_dist_neg=1.2e-38), render_ds=(), mesh_wmin=()))
+    # the edges of the brick kernels' arithmetic shortcuts (obs_fast.cuh): both ends of Params::exact_div_ok, a negative-zero
+    # truncation limit, the widest image with the float projection on, and node centres a fraction of a millimetre deep
+    cs.append(Case("E1", 512, 3.0, TUM, S1, random_poses(S1, 3, 111), color=True, noise_seed=12,
+                   params=dict(max_dist_neg=float(np.float32(1e-6)), max_dist_pos=float(np.float32(1e6))),
+                   cull_poses=random_poses(S1, 1, 911), render_ds=(2,), mesh_wmin=(0.0,)))
+    cs.append(Case("E2", 256, 3.0, TUM, S1, random_poses(S1, 4, 112), noise_seed=13,
+                   params=dict(max_dist_neg=float(np.float32(1e6)), max_weight=0.5), cull_poses=random_poses(S1, 1, 912)))
+    cs.append(Case("E3", 256, 3.0, TUM, S1, random_poses(S1, 3, 113), color=True, noise_seed=14,
+                   params=dict(max_dist_pos=-0.0, max_weight=0.0), cull_poses=random_poses(S1, 1, 913)))
+    cs.append(Case("E4", 256, 3.0, STRIP, S1, random_poses(S1, 3, 114), noise_seed=15, cull_poses=random_poses(S1, 1, 914),
+                   render_ds=(2, 4)))
+    cs.append(Case("E5", 256, 3.0, TUM, S1, [near_node_pose(p, 3.0, 3) for p in random_poses(S1, 3, 115)], noise_seed=16,
+                   params=dict(min_sensor_dist=0.0), cull_poses=random_poses(S1, 1, 915)))
     return {c.id: c for c in cs}
 
 
@@ -211,6 +236,30 @@ class EmuAdapter(OracleAdapter):
 
     def n_updates(self):
         return self.v.stats()["n_updates"]
+
+
+# ---- the edges of cases E4 and E5 ---------------------------------------------------------------------------------------------
+def view_counts(case: Case, nodes, guard):
+    """For the stored nodes and every frame of `case`, in float64: node centres in view (inside the sensor bounds and the image)
+    whose depth is below 1 mm, and in-view projections u or v that lie within `guard` of a nonzero integer (where the engine's
+    float projection defers to the double expression)."""
+    cam, p = case.cam, case.params
+    lv = nodes["keys"][:, 0].astype(np.int64)
+    ctr = -case.size / 2 + (nodes["keys"][:, 1:].astype(np.float64) + 0.5) * (case.size / np.exp2(lv))[:, None]
+    lo, hi = p.get("min_sensor_dist", 0.3), p.get("max_sensor_dist", 3.0)
+    n = dict(shallow=0, in_guard=0)
+    for pose, _ in case.frames():
+        inv = np.linalg.inv(pose)
+        pc = ctr @ inv[:3, :3].T + inv[:3, 3]
+        z = pc[:, 2]
+        ok = (z >= lo) & (z <= hi) & (z > 0)
+        u = pc[ok, 0] * cam.fx / z[ok] + cam.cx
+        v = pc[ok, 1] * cam.fy / z[ok] + cam.cy
+        inimg = (u >= 0) & (u < cam.width) & (v >= 0) & (v < cam.height)
+        n["shallow"] += int((inimg & (z[ok] < 1e-3)).sum())
+        near = lambda a: (np.abs(a - np.round(a)) <= guard) & (np.round(a) != 0)
+        n["in_guard"] += int((inimg & (near(u) | near(v))).sum())
+    return n
 
 
 # ---- exact ties (case T1) --------------------------------------------------------------------------------------------------

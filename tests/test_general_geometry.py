@@ -16,7 +16,7 @@ import pytest
 
 from oracle import oracle_py
 from tests.common import digests
-from tests.general_cases import CASES, IDS, EmuAdapter, OracleAdapter, outputs, tie_counts
+from tests.general_cases import CASES, IDS, EmuAdapter, OracleAdapter, outputs, tie_counts, view_counts
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PINS = json.load(open(os.path.join(ROOT, "tests", "golden", "general_pins.json")))["general_pin"]
@@ -96,6 +96,34 @@ def test_exact_ties_are_hit():
     assert n["proj_in_minus1_0"] >= 100, n
     assert n["points_on_planes"] >= 100_000, n
     assert n["d_new_at_limits"] >= 1000, n
+
+
+def _fused(cid):
+    a = OracleAdapter(CASES[cid])
+    for pose, cloud in CASES[cid].frames():
+        a.integrate(cloud, pose)
+    return a.dump_nodes()
+
+
+def test_edge_cases_reach_their_edges():
+    """E1-E5 exist for the limits of the brick kernels' shortcuts (tests/test_fast_arith_gpu.py tests the shortcuts alone);
+    each must keep reaching its limit, or it silently stops testing anything."""
+    from tests.test_fast_arith import probe_params
+    f32 = np.float32
+    e1 = _fused("E1")["dw"]
+    assert CASES["E1"].params == dict(max_dist_neg=float(f32(1e-6)), max_dist_pos=float(f32(1e6)))
+    assert (e1[:, 0] > 1).sum() > 100_000                                  # d_new / 1e-6: sdf far above 1
+    e2 = _fused("E2")["dw"]
+    assert ((e2[:, 0] < -0.5 / CASES["E2"].params["max_dist_neg"]) & (e2[:, 1] > 0)).sum() >= 1000   # > 0.5 m behind
+    e3 = _fused("E3")
+    assert (e3["dw"][:, 0].view(np.uint32) == 0x80000000).sum() >= 1000      # sdf = -0 stored
+    assert (e3["dw"][:, 1] == 0).all() and (e3["rgb"] != 0).any()
+    for cid in ("E1", "E2", "E3", "E4", "E5"):
+        assert probe_params(CASES[cid].config())["exact_div_ok"] == 1, cid   # the brick kernels' route
+    p4 = probe_params(CASES["E4"].config())
+    assert p4["fast_proj"] == 1 and p4["width"] == 8191
+    assert view_counts(CASES["E4"], _fused("E4"), p4["proj_guard"])["in_guard"] >= 1000
+    assert view_counts(CASES["E5"], _fused("E5"), 0.0)["shallow"] >= len(CASES["E5"].poses)   # 0 < vz < 1 mm, in view
 
 
 def test_division_overflow_case_reaches_inf():

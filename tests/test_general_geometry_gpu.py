@@ -142,3 +142,11 @@ def test_division_outside_its_exact_range_takes_the_general_kernel():
     brick = launches_per_frame(case, max_dist_neg=0.03)
     assert brick > general
     assert launches_per_frame(case, max_dist_neg=0.03, min_sensor_dist=0.0) == brick
+
+
+@pytest.mark.parametrize("cid", ["E1", "E2", "E3", "E4", "E5"])
+def test_edge_cases_take_the_brick_kernels(cid):
+    """E1-E5 test the brick kernels' shortcuts at their limits: reset() must route them to the brick kernels (more launches per
+    frame than the general depth-first kernel alone)"""
+    case = CASES[cid]
+    assert launches_per_frame(case) > launches_per_frame(case, debug_flags=1)
