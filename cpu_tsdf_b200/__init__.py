@@ -72,7 +72,7 @@ EXPORTS = [
     "b200tsdf_default_config", "b200tsdf_create", "b200tsdf_destroy", "b200tsdf_last_error",
     "b200tsdf_set_config", "b200tsdf_get_config", "b200tsdf_reset", "b200tsdf_integrate",
     "b200tsdf_integrate_device", "b200tsdf_integrate_batch_device", "b200tsdf_integrate_async",
-    "b200tsdf_comm_unique_id", "b200tsdf_comm_init", "b200tsdf_row_slice", "b200tsdf_integrate_batch_rows", "b200tsdf_gather_volume", "b200tsdf_sync", "b200tsdf_organize", "b200tsdf_integrate_unorganized", "b200tsdf_query", "b200tsdf_interpolate", "b200tsdf_render", "b200tsdf_mesh",
+    "b200tsdf_comm_unique_id", "b200tsdf_comm_init", "b200tsdf_row_slice", "b200tsdf_integrate_batch_rows", "b200tsdf_gather_volume", "b200tsdf_sync", "b200tsdf_organize", "b200tsdf_integrate_unorganized", "b200tsdf_integrate_unorganized_batch_device", "b200tsdf_query", "b200tsdf_interpolate", "b200tsdf_render", "b200tsdf_mesh",
     "b200tsdf_query_device", "b200tsdf_interpolate_device", "b200tsdf_render_batch_device",
     "b200tsdf_free", "b200tsdf_save", "b200tsdf_load", "b200tsdf_export_shard", "b200tsdf_import_shard", "b200tsdf_voxel_center", "b200tsdf_voxel_index",
     "b200tsdf_voxel_centers", "b200tsdf_occupied_voxel_indices", "b200tsdf_is_empty",
@@ -119,6 +119,8 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_meshpost_last_error.restype = C.c_char_p
     lib.b200tsdf_organize.argtypes = [vp, vp, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.POINTER(OrganizeOpts), vp, C.c_size_t, C.c_int, C.POINTER(C.c_int64)]
     lib.b200tsdf_integrate_unorganized.argtypes = [vp, vp, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.POINTER(OrganizeOpts), vp]
+    lib.b200tsdf_integrate_unorganized_batch_device.argtypes = [vp, C.c_int, vp, C.POINTER(C.c_size_t), C.c_size_t, C.c_int, C.c_int,
+                                                                C.POINTER(OrganizeOpts), vp]
     lib.b200tsdf_query.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.b200tsdf_interpolate.argtypes = [vp, vp, C.c_int, vp, vp]
     lib.b200tsdf_render.argtypes = [vp, vp, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, vp]
@@ -365,6 +367,26 @@ class TSDFVolumeOctree:
         pose = _pose(trans)
         self._check(self._lib.b200tsdf_integrate_unorganized(self._h, _ptr(pts), pts.shape[0], pts.shape[1] * 4, 0,
                                                              16 if pts.shape[1] >= 5 else -1, C.byref(opts), _ptr(pose)))
+        return True
+
+    def integrateUnorganizedBatchDevice(self, d_ptrs, counts, stride: int, poses, rgba_off: int = -1, cloud_units=1.0,
+                                        zero_nans=False, worlds_to_camera=None) -> bool:
+        """len(d_ptrs) consecutive integrateUnorganizedCloud calls on device-resident unorganised clouds (integer device pointers,
+        counts[i] points of `stride` bytes each, xyz at 0, colour bytes at rgba_off or -1), with the same result: one record upload
+        and one graph launch per 32 frames.  worlds_to_camera: None or one 4x4 world -> camera matrix per cloud.  Asynchronous."""
+        n = len(d_ptrs)
+        if len(counts) != n or len(poses) != n:
+            raise ValueError("one count and one pose per cloud")
+        arr = (C.c_void_p * max(n, 1))(*[C.c_void_p(int(x) if x else None) for x in d_ptrs])
+        cnt = (C.c_size_t * max(n, 1))(*[int(c) for c in counts])
+        ps = np.ascontiguousarray(np.stack([_pose(t) for t in poses]) if n else np.zeros((0, 4, 4)), dtype=np.float64)
+        tf = None
+        if worlds_to_camera is not None:
+            tf = np.ascontiguousarray(np.asarray(worlds_to_camera, dtype=np.float64).reshape(-1, 4, 4))
+            if len(tf) != n:
+                raise ValueError("one world -> camera matrix per cloud")
+        opts = OrganizeOpts(float(cloud_units), int(bool(zero_nans)), None if tf is None else tf.ctypes.data)
+        self._check(self._lib.b200tsdf_integrate_unorganized_batch_device(self._h, n, arr, cnt, stride, 0, rgba_off, C.byref(opts), _ptr(ps)))
         return True
 
     def _query(self, pts, what, mode):

@@ -83,6 +83,13 @@ constexpr int FRAME_RING = 64;  // per-frame records in flight (device ring + it
 constexpr int BATCH_SEGS = 16;  // host staging segments of the batch path
 constexpr int RENDER_CHUNK = 32;  // poses per render launch (blockIdx.z)
 constexpr int RENDER_SEGS = 8;    // pinned staging segments of RENDER_CHUNK render records
+// A batch of m unorganised clouds has an organise block right behind its m frame records (OrgBatch, then m OrgRecs), so both
+// go to the device in one copy; BRING_SPAN = FrameRec slots per record half (device) and per staging segment (host).
+static_assert (FRAME_RING / 2 == ORG_MAX_FRAMES, "an organise batch is one record half");
+constexpr size_t ORG_HDR = (sizeof (OrgBatch) + 15) & ~(size_t) 15;
+constexpr int BRING_SPAN = FRAME_RING / 2 + (int) ((ORG_HDR + ORG_MAX_FRAMES * sizeof (OrgRec) + sizeof (FrameRec) - 1) / sizeof (FrameRec));
+OrgBatch* org_block (FrameRec* recs, int m) { return reinterpret_cast<OrgBatch*> (recs + m); }
+OrgRec* org_recs (FrameRec* recs, int m) { return reinterpret_cast<OrgRec*> (reinterpret_cast<unsigned char*> (recs + m) + ORG_HDR); }
 
 // ---------------------------------------------------------------------------------------------
 // kernels
@@ -634,10 +641,15 @@ struct b200tsdf
   // (half, batch size); a graph is valid until the next reset()
   // device slots: two halves of FRAME_RING / 2 records, reused in stream order; host staging: BATCH_SEGS segments written round
   // robin — the host only waits when it is BATCH_SEGS batches ahead of the device
+  // (each half and each segment is BRING_SPAN slots: the frame records, then the organise block of an unorganised batch)
   FrameRec* d_bring = nullptr; FrameRec* h_bring = nullptr; int bring_half = 0; int bring_seg = 0; bool bring_used[BATCH_SEGS] = {};
   cudaEvent_t ev_bring[BATCH_SEGS] = {};
   cudaEvent_t ev_half_done[2] = { nullptr, nullptr }; bool half_used[2] = { false, false };
   cudaGraphExec_t batch_exec[2][FRAME_RING / 2 + 1] = {};
+  cudaGraphExec_t unorg_exec[2][FRAME_RING / 2 + 1] = {};   // the same with the three organise launches in front
+  // unorganised batches: the keys, filled counters and 16-byte organised images of one record half (organise and fuse of both
+  // halves run on `stream`, so one set serves both); allocated at the first unorganised integrate, freed by reset() and destroy
+  unsigned char* d_org = nullptr;
   // multi-GPU (multigpu.cuh): NCCL communicator (opaque here), row-sliced uploads
   void* comm = nullptr; int comm_rank = 0, comm_size = 1;
   unsigned char* d_rows_raw[2] = { nullptr, nullptr }; unsigned char* d_rows_full[2] = { nullptr, nullptr };
@@ -724,7 +736,10 @@ void drop_batch_graphs (b200tsdf* h)
 {
   for (int a = 0; a < 2; ++a)
     for (int n = 0; n <= FRAME_RING / 2; ++n)
+    {
       if (h->batch_exec[a][n]) { cudaGraphExecDestroy (h->batch_exec[a][n]); h->batch_exec[a][n] = nullptr; }
+      if (h->unorg_exec[a][n]) { cudaGraphExecDestroy (h->unorg_exec[a][n]); h->unorg_exec[a][n] = nullptr; }
+    }
 }
 
 int check_device_err (b200tsdf* h)
@@ -861,8 +876,8 @@ int b200tsdf_create (const b200tsdf_config* cfg, b200tsdf_t** out)
          && cudaHostAlloc (&h->h_ring, FRAME_RING * sizeof (FrameRec), cudaHostAllocDefault) == cudaSuccess
          && cudaEventCreateWithFlags (&h->ev_ring[0], cudaEventDisableTiming) == cudaSuccess
          && cudaEventCreateWithFlags (&h->ev_ring[1], cudaEventDisableTiming) == cudaSuccess
-         && cudaMalloc (&h->d_bring, FRAME_RING * sizeof (FrameRec)) == cudaSuccess
-         && cudaHostAlloc (&h->h_bring, (size_t) BATCH_SEGS * (FRAME_RING / 2) * sizeof (FrameRec), cudaHostAllocDefault) == cudaSuccess
+         && cudaMalloc (&h->d_bring, 2 * BRING_SPAN * sizeof (FrameRec)) == cudaSuccess
+         && cudaHostAlloc (&h->h_bring, (size_t) BATCH_SEGS * BRING_SPAN * sizeof (FrameRec), cudaHostAllocDefault) == cudaSuccess
          && cudaEventCreateWithFlags (&h->ev_rows_done[0], cudaEventDisableTiming) == cudaSuccess
          && cudaEventCreateWithFlags (&h->ev_rows_done[1], cudaEventDisableTiming) == cudaSuccess;
   for (int i = 0; ok && i < BATCH_SEGS; ++i) ok = cudaEventCreateWithFlags (&h->ev_bring[i], cudaEventDisableTiming) == cudaSuccess;
@@ -908,6 +923,7 @@ void b200tsdf_destroy (b200tsdf_t* h)
     if (h->ev_rows_done[i]) cudaEventDestroy (h->ev_rows_done[i]);
   }
   cudaFree (h->d_bring); if (h->h_bring) cudaFreeHost (h->h_bring);
+  cudaFree (h->d_org);
   cudaFree (h->d_rrec); if (h->h_rrec) cudaFreeHost (h->h_rrec);
   for (int i = 0; i < RENDER_SEGS; ++i) if (h->ev_rrec[i]) cudaEventDestroy (h->ev_rrec[i]);
   for (int i = 0; i < BATCH_SEGS; ++i) if (h->ev_bring[i]) cudaEventDestroy (h->ev_bring[i]);
@@ -960,6 +976,7 @@ int b200tsdf_reset (b200tsdf_t* h)
   CK (cudaStreamSynchronize (h->stream));
   CK (cudaStreamSynchronize (h->copy_stream));
   drop_batch_graphs (h);                                   // captured launches carry the old configuration
+  cudaFree (h->d_org); h->d_org = nullptr;                 // (sized by the old image size; the graphs that used it are gone)
   for (int i = 0; i < BATCH_SEGS; ++i) h->bring_used[i] = false;
   h->half_used[0] = h->half_used[1] = false;
   if (pool != h->pool || root_n != h->root_n || color != h->alloc_color || var != h->alloc_var || norm != h->alloc_norm)
@@ -1115,14 +1132,19 @@ static void fill_rec (b200tsdf* h, FrameRec& r, const unsigned char* d_pts, size
 
 // the launches of one frame; every kernel reads the frame from *d_rec, so the launches can be captured and replayed.
 // with_events: bracket the dominant kernel with an event pair of the ring (never inside a capture)
-static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, bool with_events)
+// front_pdl: k_front reads the frame's cloud before its griddepcontrol.wait, so it may only overlap the kernel before it when
+// that kernel did not write the cloud.  After the organise launches of an unorganised batch it is a plain launch (a full
+// dependency on the gather that wrote the images).
+static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, bool with_events, bool front_pdl = true)
 {
   const Params& p = h->p;
   const int npix = h->cfg.image_width * h->cfg.image_height;   // (every frame has this size: check_cloud_layout)
   const int ncells = 1 << (3 * p.C);
   {
     const int cull_blocks = (ncells + 255) / 256;
-    CK (launch_pdl (k_front, dim3 (cull_blocks + (npix + 255) / 256), dim3 (256), s, p, d_rec, cull_blocks, h->d_culled, h->d_count, h->Q.q[0], h->d_stats));
+    const dim3 grid (cull_blocks + (npix + 255) / 256);
+    if (front_pdl) CK (launch_pdl (k_front, grid, dim3 (256), s, p, d_rec, cull_blocks, h->d_culled, h->d_count, h->Q.q[0], h->d_stats));
+    else k_front<<<grid, 256, 0, s>>> (p, d_rec, cull_blocks, h->d_culled, h->d_count, h->Q.q[0], h->d_stats);
   }
   h->launches += 1;
   int kr = -1;
@@ -1251,40 +1273,78 @@ int b200tsdf_integrate_device (b200tsdf_t* h, const void* d_points, size_t strid
 // into one half of the device slots; (2) the captured launches of that half are replayed on the compute stream.  The row
 // path (multigpu.cuh) uploads the records on its copy stream AHEAD of the frames themselves — a record upload issued on
 // the compute stream would queue behind every frame copy already submitted to the one host-to-device copy engine.
+// ob / orecs: the organise block of an unorganised batch, which travels in the same copy behind the frame records
 static int batch_records (b200tsdf* h, int m, const void* const* d_points, size_t stride, int xyz_off, int rgba_off, int width, int height,
-                          const double* poses_c2w, cudaStream_t rec_stream)
+                          const double* poses_c2w, cudaStream_t rec_stream, const OrgBatch* ob = nullptr, const OrgRec* orecs = nullptr)
 {
-  constexpr int HALF = FRAME_RING / 2;
   const int a = h->bring_half, sg = h->bring_seg;
   if (h->bring_used[sg]) CK (cudaEventSynchronize (h->ev_bring[sg]));    // the copy that last read this staging segment has run
-  FrameRec* recs = h->h_bring + (size_t) sg * HALF;
+  FrameRec* recs = h->h_bring + (size_t) sg * BRING_SPAN;
   for (int i = 0; i < m; ++i)
   {
     if (!d_points[i]) return h->fail (B200TSDF_EINVAL, "null cloud in batch");
     fill_rec (h, recs[i], (const unsigned char*) d_points[i], stride, xyz_off, rgba_off, width, height, poses_c2w + 16 * (size_t) i);
   }
+  size_t bytes = (size_t) m * sizeof (FrameRec);
+  if (ob)
+  {
+    *org_block (recs, m) = *ob;
+    std::memcpy (org_recs (recs, m), orecs, (size_t) m * sizeof (OrgRec));
+    bytes += ORG_HDR + (size_t) m * sizeof (OrgRec);
+  }
   // the device half is rewritten only after the launches that last read it (other stream: wait for their event)
   if (rec_stream != h->stream && h->half_used[a]) CK (cudaStreamWaitEvent (rec_stream, h->ev_half_done[a], 0));
-  CK (cudaMemcpyAsync (h->d_bring + a * HALF, recs, (size_t) m * sizeof (FrameRec), cudaMemcpyHostToDevice, rec_stream));
+  CK (cudaMemcpyAsync (h->d_bring + a * BRING_SPAN, recs, bytes, cudaMemcpyHostToDevice, rec_stream));
   CK (cudaEventRecord (h->ev_bring[sg], rec_stream));      // the staging segment is free again once this copy has run
   h->bring_used[sg] = true; h->bring_seg = (sg + 1) % BATCH_SEGS;
   return B200TSDF_OK;
 }
-static int batch_launch (b200tsdf* h, int m)
+// the organised images of the unorganised batch path (layout: keys HALF*npix*8 | filled counters HALF*8 | images HALF*npix*16)
+static size_t org_npix (const b200tsdf* h) { return (size_t) h->cfg.image_width * h->cfg.image_height; }
+static unsigned long long* org_keys (const b200tsdf* h) { return reinterpret_cast<unsigned long long*> (h->d_org); }
+static unsigned long long* org_filled (const b200tsdf* h) { return org_keys (h) + ORG_MAX_FRAMES * org_npix (h); }
+static unsigned char* org_images (const b200tsdf* h) { return h->d_org + ORG_MAX_FRAMES * org_npix (h) * 8 + 256; }
+static int org_buffers (b200tsdf* h)
 {
-  constexpr int HALF = FRAME_RING / 2;
+  if (h->d_org) return B200TSDF_OK;
+  const size_t bytes = ORG_MAX_FRAMES * org_npix (h) * (8 + 16) + 256;
+  if (cudaMalloc (&h->d_org, bytes) != cudaSuccess) { h->d_org = nullptr; return alloc_failed (h, "organised images of an unorganised batch"); }
+  return B200TSDF_OK;
+}
+
+// the three organise launches of m frames (organize.cuh): keys cleared, every point z-buffered, m images gathered
+static int launch_organize (b200tsdf* h, cudaStream_t s, const OrgBatch* d_ob, const OrgRec* d_recs, int m,
+                            unsigned long long* zkey, unsigned long long* filled, unsigned char* out)
+{
+  const int npix = (int) org_npix (h);
+  const dim3 pix_grid ((npix + 255) / 256, m);
+  k_org_clear<<<pix_grid, 256, 0, s>>> (zkey, npix, filled);
+  k_org_zmin<<<h->sm_count * 8, 256, 0, s>>> (d_ob, d_recs, m, npix, zkey);
+  k_org_gather<<<pix_grid, 256, 0, s>>> (d_ob, d_recs, npix, zkey, out, filled);
+  h->launches += 3;
+  CK (cudaGetLastError ());
+  return B200TSDF_OK;
+}
+
+// organize: the records carry the organise block of an unorganised batch (batch_records), whose three launches come first
+static int batch_launch (b200tsdf* h, int m, bool organize = false)
+{
   cudaStream_t s = h->stream;
   const int a = h->bring_half;
-  cudaGraphExec_t& exec = h->batch_exec[a][m];          // (nothing of a frame is baked into the launches: they read the record)
+  FrameRec* const d_recs = h->d_bring + a * BRING_SPAN;
+  cudaGraphExec_t& exec = (organize ? h->unorg_exec : h->batch_exec)[a][m];   // (nothing of a frame is baked into the launches: they read the record)
+  const int org_launches = organize ? 3 : 0;
   if (!exec)
   {
     const long long l0 = h->launches, f0 = h->prof_frames;
     cudaGraph_t g = nullptr;
     CK (cudaStreamBeginCapture (s, cudaStreamCaptureModeThreadLocal));
     int rc = B200TSDF_OK;
-    for (int i = 0; i < m && rc == B200TSDF_OK; ++i) rc = launch_frame (h, s, h->d_bring + a * HALF + i, false);
+    if (organize) rc = launch_organize (h, s, org_block (d_recs, m), org_recs (d_recs, m), m, org_keys (h), org_filled (h), org_images (h));
+    // (the first k_front of an unorganised batch reads what the gather wrote: no programmatic overlap with it, see launch_frame)
+    for (int i = 0; i < m && rc == B200TSDF_OK; ++i) rc = launch_frame (h, s, d_recs + i, false, !(organize && i == 0));
     cudaError_t ce = cudaStreamEndCapture (s, &g);
-    h->launches_per_frame = (int) ((h->launches - l0) / std::max (1, m));
+    h->launches_per_frame = (int) ((h->launches - l0 - org_launches) / std::max (1, m));
     h->launches = l0; h->prof_frames = f0;
     if (rc) { if (g) cudaGraphDestroy (g); return rc; }
     if (ce != cudaSuccess) return h->fail (B200TSDF_ECUDA, std::string ("graph capture: ") + cudaGetErrorString (ce));
@@ -1297,7 +1357,7 @@ static int batch_launch (b200tsdf* h, int m)
   h->half_used[a] = true;
   note_device_err (h, s);
   h->bring_half ^= 1;
-  h->launches += (long long) m * h->launches_per_frame; h->graph_launches++;
+  h->launches += org_launches + (long long) m * h->launches_per_frame; h->graph_launches++;
   h->prof_frames += m;
   h->timed = false;
   h->is_empty = false;
@@ -1435,45 +1495,77 @@ int b200tsdf_integrate_async (b200tsdf_t* h, const void* points, size_t stride, 
 { return integrate_host (h, points, stride, xyz_off, rgba_off, width, height, pose, false); }
 
 // ---- unorganised clouds (integrate.cpp:548-635) ------------------------------------------------
+// Every organise goes through the batched kernels of organize.cuh: b200tsdf_organize is a batch of one frame written in the
+// caller's layout, b200tsdf_integrate_unorganized an upload plus a batch of one, and the batch entry point m frames per record
+// half, each half one graph launch.
 namespace {
 
-// uploads the points, z-buffers them and writes the organized cloud to d_out (device).  Scratch layout:
-// [points n*stride | zkey npix*8 | filled counter 8 | organized npix*out_stride (when d_out == nullptr)]
-int organize_on_device (b200tsdf* h, const void* points, size_t n, size_t stride, int xyz_off, int rgba_off,
-                        const b200tsdf_organize_opts* opts, size_t out_stride, int out_rgba_off,
-                        unsigned char** d_out, unsigned long long** d_filled)
+// the checks every organise entry point applies to its input points (org_load reads them as floats: 4-byte aligned)
+int org_args (b200tsdf* h, size_t stride, int xyz_off, int rgba_off, const b200tsdf_organize_opts* opts)
 {
-  if (!h || (!points && n) || !opts) return B200TSDF_EINVAL;
+  if (!opts) return B200TSDF_EINVAL;
   if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "organize before reset() (the image size and intrinsics are read at reset)");
-  if (stride < 12 || xyz_off < 0 || (size_t) xyz_off + 12 > stride || (rgba_off >= 0 && (size_t) rgba_off + 4 > stride))
-    return h->fail (B200TSDF_EINVAL, "bad point layout");
-  if (out_stride < 16 || (out_stride & 3) || (out_rgba_off >= 0 && ((size_t) out_rgba_off + 4 > out_stride || out_rgba_off < 12)))
-    return h->fail (B200TSDF_EINVAL, "bad organized layout");
+  if (stride < 12 || (stride & 3) || xyz_off < 0 || (xyz_off & 3) || (size_t) xyz_off + 12 > stride
+      || (rgba_off >= 0 && ((size_t) rgba_off + 4 > stride || (rgba_off & 3))))
+    return h->fail (B200TSDF_EINVAL, "bad point layout (need 4-byte aligned stride, xyz_off and rgba_off, xyz_off + 12 <= stride and rgba_off + 4 <= stride)");
+  return B200TSDF_OK;
+}
+
+int org_count (b200tsdf* h, const void* points, size_t n)
+{
+  if (!points && n) return h->fail (B200TSDF_EINVAL, "null cloud with points");
   if (n >= (1ull << 32)) return h->fail (B200TSDF_EINVAL, "more than 2^32-1 points in one cloud");
-  cudaSetDevice (h->device);
-  OrgParams o{};
+  return B200TSDF_OK;
+}
+
+OrgBatch org_batch (const b200tsdf* h, const b200tsdf_organize_opts* opts, size_t stride, int xyz_off, int rgba_off,
+                    size_t out_stride, int out_rgba_off)
+{
+  OrgBatch b{};
   // the program keeps its intrinsics as float globals (integrate.cpp:63-68, 349-361)
-  o.fx = (float) h->cfg.fx; o.fy = (float) h->cfg.fy; o.cx = (float) h->cfg.cx; o.cy = (float) h->cfg.cy;
-  o.width = h->cfg.image_width; o.height = h->cfg.image_height;
-  o.cloud_units = opts->cloud_units; o.zero_nans = opts->zero_nans; o.has_tf = opts->world_to_camera != nullptr;
-  if (o.has_tf) for (int i = 0; i < 12; ++i) o.tf[i] = opts->world_to_camera[i];
-  size_t npix = (size_t) o.width * o.height;
-  size_t off_key = (n * stride + 255) & ~(size_t) 255, off_cnt = off_key + npix * 8, off_out = off_cnt + 256;
-  { int rc = h->scratch (off_out + npix * out_stride + 64); if (rc) return rc; }
-  unsigned char* d_pts = h->d_scratch;
-  unsigned long long* zkey = (unsigned long long*) (h->d_scratch + off_key);
-  *d_filled = (unsigned long long*) (h->d_scratch + off_cnt);
-  *d_out = h->d_scratch + off_out;
-  cudaStream_t s = h->stream;
-  if (n) { CK (cudaMemcpyAsync (d_pts, points, n * stride, cudaMemcpyHostToDevice, s)); h->h2d_bytes += (long long) (n * stride); }
-  k_org_clear<<<(unsigned) ((npix + 255) / 256), 256, 0, s>>> (zkey, (int) npix, *d_filled);
-  if (n)
+  b.o.fx = (float) h->cfg.fx; b.o.fy = (float) h->cfg.fy; b.o.cx = (float) h->cfg.cx; b.o.cy = (float) h->cfg.cy;
+  b.o.width = h->cfg.image_width; b.o.height = h->cfg.image_height;
+  b.o.cloud_units = opts->cloud_units; b.o.zero_nans = opts->zero_nans;
+  b.stride = stride; b.xyz_off = xyz_off; b.rgba_off = rgba_off;
+  b.out_stride = out_stride; b.out_rgba_off = out_rgba_off;
+  return b;
+}
+
+// w2c: a row-major 4x4 world -> camera matrix or null
+OrgRec org_rec (const void* d_pts, size_t n, unsigned long long first, const double* w2c)
+{
+  OrgRec r{};
+  r.pts = static_cast<const unsigned char*> (d_pts); r.count = n; r.first = first;
+  r.has_tf = w2c != nullptr;
+  if (w2c) for (int i = 0; i < 12; ++i) r.tf[i] = w2c[i];
+  return r;
+}
+
+// n frames, HALF per record half: the organised images are 16-byte pixels {x, y, z, bgra} in d_org, fused like an organised
+// batch (stride 16, xyz at 0, colour at 12).  The arguments have been checked.
+int unorganized_batches (b200tsdf* h, int n, const void* const* d_points, const size_t* counts, size_t stride, int xyz_off, int rgba_off,
+                         const b200tsdf_organize_opts* opts, const double* poses_c2w)
+{
+  constexpr int HALF = FRAME_RING / 2;
+  if (int rc = org_buffers (h)) return rc;
+  const OrgBatch ob = org_batch (h, opts, stride, xyz_off, rgba_off, 16, 12);
+  const size_t npix = org_npix (h);
+  for (int done = 0; done < n;)
   {
-    size_t blocks = std::min<size_t> ((n + 255) / 256, (size_t) h->sm_count * 16);
-    k_org_zmin<<<(unsigned) blocks, 256, 0, s>>> (o, d_pts, n, stride, xyz_off, zkey);
+    const int m = std::min (HALF, n - done);
+    const void* imgs[HALF]; OrgRec recs[HALF];
+    unsigned long long first = 0;
+    for (int i = 0; i < m; ++i)
+    {
+      const int k = done + i;
+      imgs[i] = org_images (h) + (size_t) i * npix * 16;
+      recs[i] = org_rec (d_points[k], counts[k], first, opts->world_to_camera ? opts->world_to_camera + 16 * (size_t) k : nullptr);
+      first += counts[k];
+    }
+    if (int rc = batch_records (h, m, imgs, 16, 0, 12, h->cfg.image_width, h->cfg.image_height, poses_c2w + 16 * (size_t) done, h->stream, &ob, recs)) return rc;
+    if (int rc = batch_launch (h, m, true)) return rc;
+    done += m;
   }
-  k_org_gather<<<(unsigned) ((npix + 255) / 256), 256, 0, s>>> (o, d_pts, stride, xyz_off, rgba_off, zkey, *d_out, out_stride, out_rgba_off, *d_filled);
-  h->launches += n ? 3 : 2;
   CK (cudaGetLastError ());
   return B200TSDF_OK;
 }
@@ -1484,15 +1576,32 @@ int b200tsdf_organize (b200tsdf_t* h, const void* points, size_t n, size_t strid
                        const b200tsdf_organize_opts* opts, void* out, size_t out_stride, int out_rgba_off, int64_t* n_filled)
 {
   if (!h || !out) return B200TSDF_EINVAL;
-  unsigned char* d_out = nullptr; unsigned long long* d_filled = nullptr;
-  int rc = organize_on_device (h, points, n, stride, xyz_off, rgba_off, opts, out_stride, out_rgba_off, &d_out, &d_filled);
-  if (rc) return rc;
-  size_t bytes = (size_t) h->cfg.image_width * h->cfg.image_height * out_stride;
+  if (int rc = org_args (h, stride, xyz_off, rgba_off, opts)) return rc;
+  if (int rc = org_count (h, points, n)) return rc;
+  if (out_stride < 16 || (out_stride & 3) || (out_rgba_off >= 0 && ((size_t) out_rgba_off + 4 > out_stride || out_rgba_off < 12)))
+    return h->fail (B200TSDF_EINVAL, "bad organized layout");
+  cudaSetDevice (h->device);
+  const size_t npix = org_npix (h);
+  // scratch: [organise block | points n*stride | zkey npix*8 | filled counter 8 | organized npix*out_stride]
+  const size_t off_pts = (ORG_HDR + sizeof (OrgRec) + 255) & ~(size_t) 255, off_key = (off_pts + n * stride + 255) & ~(size_t) 255, off_cnt = off_key + npix * 8, off_out = off_cnt + 256;
+  { int rc = h->scratch (off_out + npix * out_stride + 64); if (rc) return rc; }
+  unsigned char* d = h->d_scratch;
+  unsigned char hdr[ORG_HDR + sizeof (OrgRec)];
+  const OrgBatch ob = org_batch (h, opts, stride, xyz_off, rgba_off, out_stride, out_rgba_off);
+  const OrgRec rec = org_rec (d + off_pts, n, 0, opts->world_to_camera);
+  std::memcpy (hdr, &ob, sizeof (ob)); std::memcpy (hdr + ORG_HDR, &rec, sizeof (rec));
+  cudaStream_t s = h->stream;
+  CK (cudaMemcpyAsync (d, hdr, sizeof (hdr), cudaMemcpyHostToDevice, s));          // (pageable: staged before the call returns)
+  if (n) { CK (cudaMemcpyAsync (d + off_pts, points, n * stride, cudaMemcpyHostToDevice, s)); h->h2d_bytes += (long long) (n * stride); }
+  unsigned long long* d_filled = (unsigned long long*) (d + off_cnt);
+  if (int rc = launch_organize (h, s, (const OrgBatch*) d, (const OrgRec*) (d + ORG_HDR), 1, (unsigned long long*) (d + off_key), d_filled, d + off_out))
+    return rc;
+  const size_t bytes = npix * out_stride;
   unsigned long long filled = 0;
   // bytes of a pixel that the layout does not name (padding) are zero in the result
-  CK (cudaMemcpyAsync (out, d_out, bytes, cudaMemcpyDeviceToHost, h->stream));
-  CK (cudaMemcpyAsync (&filled, d_filled, 8, cudaMemcpyDeviceToHost, h->stream));
-  CK (cudaStreamSynchronize (h->stream));
+  CK (cudaMemcpyAsync (out, d + off_out, bytes, cudaMemcpyDeviceToHost, s));
+  CK (cudaMemcpyAsync (&filled, d_filled, 8, cudaMemcpyDeviceToHost, s));
+  CK (cudaStreamSynchronize (s));
   h->d2h_bytes += (long long) bytes + 8;
   if (n_filled) *n_filled = (int64_t) filled;
   return B200TSDF_OK;
@@ -1502,11 +1611,28 @@ int b200tsdf_integrate_unorganized (b200tsdf_t* h, const void* points, size_t n,
                                     const b200tsdf_organize_opts* opts, const double* pose)
 {
   if (!h || !pose) return B200TSDF_EINVAL;
-  unsigned char* d_out = nullptr; unsigned long long* d_filled = nullptr;
-  // organized pixels are 16 bytes in HBM: x, y, z, then the colour bytes b,g,r,a
-  int rc = organize_on_device (h, points, n, stride, xyz_off, rgba_off, opts, 16, 12, &d_out, &d_filled);
-  if (rc) return rc;
-  return integrate_on_device (h, d_out, 16, 0, 12, h->cfg.image_width, h->cfg.image_height, pose);
+  if (int rc = org_args (h, stride, xyz_off, rgba_off, opts)) return rc;
+  if (int rc = org_count (h, points, n)) return rc;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  // the points go to the scratch on the handle's stream (after the launches that last read it), then a batch of one
+  { int rc = h->scratch (n * stride + 64); if (rc) return rc; }
+  if (n) { CK (cudaMemcpyAsync (h->d_scratch, points, n * stride, cudaMemcpyHostToDevice, h->stream)); h->h2d_bytes += (long long) (n * stride); }
+  const void* d_pts = h->d_scratch;
+  return unorganized_batches (h, 1, &d_pts, &n, stride, xyz_off, rgba_off, opts, pose);
+}
+
+int b200tsdf_integrate_unorganized_batch_device (b200tsdf_t* h, int n, const void* const* d_points, const size_t* counts,
+                                                 size_t stride, int xyz_off, int rgba_off,
+                                                 const b200tsdf_organize_opts* opts, const double* poses_c2w)
+{
+  if (!h || n < 0 || (n && (!d_points || !counts || !poses_c2w))) return B200TSDF_EINVAL;
+  if (int rc = org_args (h, stride, xyz_off, rgba_off, opts)) return rc;
+  for (int i = 0; i < n; ++i) if (int rc = org_count (h, d_points[i], counts[i])) return rc;   // (nothing is enqueued for a refused batch)
+  if (!n) return B200TSDF_OK;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  return unorganized_batches (h, n, d_points, counts, stride, xyz_off, rgba_off, opts, poses_c2w);
 }
 
 int b200tsdf_sync (b200tsdf_t* h)

@@ -7,10 +7,14 @@
 // :216-222), so its IEEE bit pattern orders like the value and one 64-bit atomicMin per point
 // on the key (z bits << 32 | index) reproduces the sequential result exactly and in any order.
 //
-//   k_org_clear   zkey[pixel] = ~0
-//   k_org_zmin    one thread per point: units, zero->NaN, world->camera, project, atomicMin
-//   k_org_gather  one thread per pixel: recompute the winner's point and write it (or the
-//                 default point with z = NaN)
+// A batch of m clouds is organised by three launches, whatever m is.  Nothing of a frame is a launch argument: the
+// shared block (OrgBatch) and one record per frame (OrgRec) sit in device memory, so the launches can be captured once
+// into a CUDA graph and replayed on other clouds, other counts and other options.
+//   k_org_clear   zkey[frame][pixel] = ~0, filled[frame] = 0
+//   k_org_zmin    a grid-stride loop over the batch's concatenated points: the frame from the prefix offsets, then
+//                 units, zero->NaN, world->camera, project, atomicMin on the key of (z, index within the frame)
+//   k_org_gather  one thread per pixel of each frame: recompute the winner's point and write it (or the default point
+//                 with z = NaN)
 #pragma once
 #include "tsdf_core.cuh"
 #include <cstring>
@@ -94,44 +98,116 @@ B2_HD void org_emit (const OrgParams& o, const unsigned char* pts, size_t stride
   if (out_rgba_off >= 0) { unsigned char* d = out + out_rgba_off; d[0] = c[0]; d[1] = c[1]; d[2] = c[2]; d[3] = c[3]; }
 }
 
-#ifdef __CUDACC__
-__global__ void k_org_clear (unsigned long long* __restrict__ zkey, int npix, unsigned long long* __restrict__ n_filled)
+// ---- batches ---------------------------------------------------------------------------------------
+constexpr int ORG_MAX_FRAMES = 32;       // frames per organise batch (one record half of the batch path)
+
+// what every frame of a batch shares (device memory, one block per batch)
+struct OrgBatch
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < npix) zkey[i] = ~0ull;
-  if (i == 0) *n_filled = 0ull;
+  OrgParams o;                   // intrinsics, image size, units, zero_nans; has_tf / tf are per frame (OrgRec)
+  unsigned long long stride;     // input points: `stride` bytes each, xyz at xyz_off, colour bytes at rgba_off or -1
+  int xyz_off, rgba_off;
+  unsigned long long out_stride; // organised pixels: xyz at 0, colour bytes at out_rgba_off or -1 (see org_emit)
+  int out_rgba_off, pad_;
+};
+
+// one frame of a batch (device memory)
+struct OrgRec
+{
+  const unsigned char* pts;      // the frame's points (may be null when count == 0)
+  unsigned long long count;      // number of points (< 2^32: the key keeps the index within the frame in 32 bits)
+  unsigned long long first;      // flat index of the frame's first point in the batch's concatenation (prefix sum of count)
+  int has_tf, pad_;
+  double tf[12];                 // world -> camera rows 0..2 when has_tf
+};
+
+// the parameters org_prepare / org_pixel / org_emit take for frame r of batch b
+B2_HD OrgParams org_frame_params (const OrgBatch& b, const OrgRec& r)
+{
+  OrgParams o = b.o;
+  o.has_tf = r.has_tf;
+  for (int i = 0; i < 12; ++i) o.tf[i] = r.tf[i];
+  return o;
 }
 
-__global__ void k_org_zmin (OrgParams o, const unsigned char* __restrict__ pts, size_t n, size_t stride, int xyz_off,
+// the frame of flat point index k (k < first[m-1] + count[m-1]): the last frame whose first point is at or before k.  A frame
+// without points has the same offset as the frame after it and is never chosen.
+B2_HD int org_frame_of (const unsigned long long* first, int m, unsigned long long k)
+{
+  int lo = 0, hi = m - 1;
+  while (lo < hi)
+  {
+    const int mid = (lo + hi + 1) >> 1;
+    if (first[mid] <= k) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+#ifdef __CUDACC__
+// grid (pixel blocks, m)
+__global__ void k_org_clear (unsigned long long* __restrict__ zkey, int npix, unsigned long long* __restrict__ n_filled)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < npix) zkey[(size_t) blockIdx.y * npix + i] = ~0ull;
+  if (i == 0) n_filled[blockIdx.y] = 0ull;
+}
+
+// persistent grid (its size depends only on the device): every point of the batch, frame found from the prefix offsets
+__global__ void k_org_zmin (const OrgBatch* __restrict__ gb, const OrgRec* __restrict__ recs, int m, int npix,
                             unsigned long long* __restrict__ zkey)
 {
-  for (size_t j = (size_t) blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (size_t) gridDim.x * blockDim.x)
+  __shared__ OrgParams s_o[ORG_MAX_FRAMES];
+  __shared__ const unsigned char* s_pts[ORG_MAX_FRAMES];
+  __shared__ unsigned long long s_first[ORG_MAX_FRAMES];
+  __shared__ unsigned long long s_total;
+  __shared__ unsigned long long s_stride;
+  __shared__ int s_xyz_off;
+  for (int f = threadIdx.x; f < m; f += blockDim.x)
   {
+    s_o[f] = org_frame_params (*gb, recs[f]);
+    s_pts[f] = recs[f].pts; s_first[f] = recs[f].first;
+  }
+  if (threadIdx.x == 0) { s_total = recs[m - 1].first + recs[m - 1].count; s_stride = gb->stride; s_xyz_off = gb->xyz_off; }
+  __syncthreads ();
+  const unsigned long long total = s_total;
+  for (unsigned long long k = (unsigned long long) blockIdx.x * blockDim.x + threadIdx.x; k < total; k += (unsigned long long) gridDim.x * blockDim.x)
+  {
+    const int f = org_frame_of (s_first, m, k);
+    const unsigned long long j = k - s_first[f];           // the index within its frame: ties go to its earliest point
+    const OrgParams& o = s_o[f];
     float x, y, z;
-    org_load (pts, stride, xyz_off, j, x, y, z);
+    org_load (s_pts[f], s_stride, s_xyz_off, j, x, y, z);
     org_prepare (o, x, y, z);
-    int pix = org_pixel (o, x, y, z);
+    const int pix = org_pixel (o, x, y, z);
     if (pix < 0) continue;
-    unsigned long long key = org_key (z, (unsigned int) j);
-    if (key < zkey[pix]) atomicMin (&zkey[pix], key);     // the plain read filters most losers
+    const unsigned long long key = org_key (z, (unsigned int) j);
+    unsigned long long* zk = zkey + (size_t) f * npix + pix;
+    if (key < *zk) atomicMin (zk, key);                    // the plain read filters most losers
   }
 }
 
-__global__ void k_org_gather (OrgParams o, const unsigned char* __restrict__ pts, size_t stride, int xyz_off, int rgba_off,
-                              const unsigned long long* __restrict__ zkey, unsigned char* __restrict__ out, size_t out_stride,
-                              int out_rgba_off, unsigned long long* __restrict__ n_filled)
+// grid (pixel blocks, m): frame blockIdx.y's image starts at out + frame * npix * out_stride
+__global__ void k_org_gather (const OrgBatch* __restrict__ gb, const OrgRec* __restrict__ recs, int npix,
+                              const unsigned long long* __restrict__ zkey, unsigned char* __restrict__ out,
+                              unsigned long long* __restrict__ n_filled)
 {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  int npix = o.width * o.height;
+  __shared__ OrgParams s_o;
+  __shared__ const unsigned char* s_pts;
+  const int f = blockIdx.y;
+  if (threadIdx.x == 0) { s_o = org_frame_params (*gb, recs[f]); s_pts = recs[f].pts; }
+  __syncthreads ();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
   bool filled = false;
   if (i < npix)
   {
-    unsigned long long key = zkey[i];
+    const size_t q = (size_t) f * npix + i;
+    const unsigned long long key = zkey[q];
     filled = key != ~0ull;
-    org_emit (o, pts, stride, xyz_off, rgba_off, key, out + (size_t) i * out_stride, out_stride, out_rgba_off);
+    const size_t os = gb->out_stride;
+    org_emit (s_o, s_pts, gb->stride, gb->xyz_off, gb->rgba_off, key, out + q * os, os, gb->out_rgba_off);
   }
-  unsigned m = __ballot_sync (0xffffffffu, filled);
-  if ((threadIdx.x & 31) == 0 && m) atomicAdd (n_filled, (unsigned long long) __popc (m));
+  const unsigned bal = __ballot_sync (0xffffffffu, filled);
+  if ((threadIdx.x & 31) == 0 && bal) atomicAdd (&n_filled[f], (unsigned long long) __popc (bal));
 }
 #endif
 

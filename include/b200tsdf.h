@@ -133,6 +133,19 @@ int  b200tsdf_organize (b200tsdf_t* h, const void* points, size_t n, size_t stri
 /* organise + integrateCloud without the organized cloud ever leaving HBM (integrate.cpp:582-635 + :673) */
 int  b200tsdf_integrate_unorganized (b200tsdf_t* h, const void* points, size_t n, size_t stride, int xyz_off,
                                      int rgba_off, const b200tsdf_organize_opts* opts, const double* pose_c2w);
+/* n consecutive b200tsdf_integrate_unorganized calls (cloud i, pose i, world_to_camera matrix i) on clouds resident in device
+ * memory of h's device, with the same result bit for bit.  d_points: n device pointers; counts: n point counts in host memory
+ * (0 is allowed and gives an all-NaN organised image; that cloud's pointer may then be NULL; each count < 2^32); one point
+ * layout for all (stride, xyz_off and rgba_off multiples of 4, xyz_off + 12 <= stride, rgba_off + 4 <= stride).
+ * opts->world_to_camera: NULL or n row-major 4x4 matrices back to back; cloud_units and zero_nans apply to every cloud.
+ * poses_c2w: n row-major 4x4 matrices back to back.  Every 32 frames are organised and fused by one CUDA-graph launch
+ * (captured once per batch size, replayed afterwards).  Asynchronous on the handle's stream; errors as for
+ * b200tsdf_integrate_device.  B200TSDF_EINVAL for a bad argument, B200TSDF_ESTATE before reset(), B200TSDF_ENOMEM when the
+ * organised images (32 * image_width * image_height * 24 bytes, allocated at the first unorganised integrate and freed by
+ * reset()) do not fit. */
+int  b200tsdf_integrate_unorganized_batch_device (b200tsdf_t* h, int n, const void* const* d_points, const size_t* counts,
+                                                  size_t stride, int xyz_off, int rgba_off,
+                                                  const b200tsdf_organize_opts* opts, const double* poses_c2w);
 
 /* getFxn / getGradient / getHessian (cpp:655-725) with mode 0, or the combined
  * getFxnAndGradient / getFxnGradientAndHessian (cpp:728-794) with mode 1.  what: bit0 value,

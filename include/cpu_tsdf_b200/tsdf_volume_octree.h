@@ -204,6 +204,27 @@ public:
     status_ = b200tsdf_integrate_unorganized (h_, points, n, stride, xyz_off, rgba_off, &opts, m);
     return status_ == 0;
   }
+  // integrateUnorganizedCloud for every cloud of a batch resident in device memory (d_points[i]: counts[i] records, the layout
+  // above), with the same result; poses[i] and worlds_to_camera[i] (or none) belong to cloud i.  Asynchronous on the volume's
+  // stream: every 32 clouds are organised and fused by one CUDA-graph launch.
+  bool integrateUnorganizedCloudsDevice (const std::vector<const void*>& d_points, const std::vector<std::size_t>& counts,
+                                         std::size_t stride, int xyz_off, int rgba_off, const std::vector<Affine3d>& poses,
+                                         float cloud_units = 1.f, bool zero_nans = false,
+                                         const std::vector<Affine3d>* worlds_to_camera = nullptr)
+  {
+    if (!h_) return false;
+    const std::size_t n = d_points.size ();
+    if (counts.size () != n || poses.size () != n || (worlds_to_camera && worlds_to_camera->size () != n))
+    { status_ = B200TSDF_EINVAL; return false; }
+    std::vector<double> m (16 * n), w2c (worlds_to_camera ? 16 * n : 0);
+    for (std::size_t i = 0; i < n; ++i) detail::pose_rows (poses[i], m.data () + 16 * i);
+    if (worlds_to_camera) for (std::size_t i = 0; i < n; ++i) detail::pose_rows ((*worlds_to_camera)[i], w2c.data () + 16 * i);
+    b200tsdf_organize_opts opts;
+    opts.cloud_units = cloud_units; opts.zero_nans = zero_nans ? 1 : 0; opts.world_to_camera = worlds_to_camera ? w2c.data () : nullptr;
+    status_ = b200tsdf_integrate_unorganized_batch_device (h_, static_cast<int> (n), d_points.data (), counts.data (), stride, xyz_off,
+                                                           rgba_off, &opts, m.data ());
+    return status_ == 0;
+  }
 
   bool getFxn (const PointXYZ& pt, float& val) const                                               // cpp:655-672
   { std::uint8_t ok = 0; float p[3] = { pt.x, pt.y, pt.z }; b200tsdf_query (h_, p, 1, 1, 0, &val, nullptr, nullptr, &ok); return ok != 0; }
