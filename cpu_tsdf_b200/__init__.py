@@ -79,6 +79,7 @@ EXPORTS = [
     "b200tsdf_get_stats", "b200tsdf_download_nodes", "b200tsdf_download_color_payload", "b200tsdf_frustum_cull",
     "b200tsdf_profile_begin", "b200tsdf_profile_end",
     "b200tsdf_mesh_flatten", "b200tsdf_mesh_cleanup", "b200tsdf_mesh_free", "b200tsdf_meshpost_last_error", "b200tsdf_debug_timing",
+    "b200tsdf_mesh_device", "b200tsdf_mesh_flatten_device", "b200tsdf_mesh_cleanup_device",
 ]
 
 _lib = None
@@ -128,6 +129,9 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_interpolate_device.argtypes = [vp, vp, C.c_int, vp, vp]
     lib.b200tsdf_render_batch_device.argtypes = [vp, C.c_int, vp, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, vp]
     lib.b200tsdf_mesh.argtypes = [vp, C.c_float, C.c_int, C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_size_t)]
+    lib.b200tsdf_mesh_device.argtypes = [vp, C.c_float, C.c_int, vp, vp, C.c_size_t, szp]
+    lib.b200tsdf_mesh_flatten_device.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, C.c_float, vp, vp, szp, szp]
+    lib.b200tsdf_mesh_cleanup_device.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, C.c_float, C.c_int, vp, vp, szp, szp]
     lib.b200tsdf_save.argtypes = [vp, C.c_char_p]
     lib.b200tsdf_load.argtypes = [vp, C.c_char_p]
     lib.b200tsdf_export_shard.argtypes = [vp, vp, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -619,6 +623,20 @@ class MarchingCubesTSDFOctree:
         polys = np.arange(nv, dtype=np.int32).reshape(-1, 3)
         return verts, rgb, polys
 
+    def reconstructDevice(self, d_verts: int | None = None, capacity: int = 0, d_rgb: int | None = None) -> int:
+        """reconstruct() into device memory of the volume's device (integer device pointers, e.g. a torch tensor's data_ptr()):
+        the same vertices (3 float32 each) and, when colouring by RGB or confidence and d_rgb is given, colours (3 bytes each),
+        in the same order; the polygons are {3i, 3i+1, 3i+2}.  Returns the vertex count.  d_verts=None counts only; a capacity
+        (in vertices) below the count raises and writes nothing.  Ordered after every integrate queued on the volume."""
+        v = self.tsdf_volume_
+        if v is None:
+            raise B200Error("setInputTSDF first")
+        mode = 2 if self.color_by_confidence_ else (1 if self.color_by_rgb_ else 0)
+        n = C.c_size_t()
+        dp = lambda a: None if a is None else C.c_void_p(int(a))
+        v._check(v._lib.b200tsdf_mesh_device(v._h, self.w_min_, mode, dp(d_verts), dp(d_rgb), int(capacity), C.byref(n)))
+        return n.value
+
 
 # ---- mesh post-processing of the reference's `integrate` program (src/prog/integrate.cpp:103-214) ----------
 def _meshpost(fn_name, verts, tris, *args, device=0):
@@ -647,3 +665,28 @@ def flattenVertices(verts, tris, min_dist: float = 0.0001, device: int = 0):
 def cleanupMesh(verts, tris, face_dist: float = 0.02, min_neighbors: int = 5, device: int = 0):
     """integrate.cpp:152-214: remove face clusters of at most min_neighbors faces and the vertices left unused."""
     return _meshpost("b200tsdf_mesh_cleanup", verts, tris, C.c_float(face_dist), int(min_neighbors), device=device)
+
+
+# The same two on arrays in device memory of vol's device (integer device pointers), on vol's stream.  d_tris=None: a triangle
+# soup (triangle t = {3t, 3t+1, 3t+2}, nverts == 3 * ntris).  The outputs are sized like the inputs (3 * nverts float32,
+# 3 * ntris int32) and must not overlap them; the inputs are only read.  Both return (nverts, ntris) of the result.
+def _meshpost_device(fn_name, vol, d_verts, nverts, d_tris, ntris, d_out_verts, d_out_tris, *args):
+    dp = lambda a: None if a is None else C.c_void_p(int(a))
+    nv, nt = C.c_size_t(0), C.c_size_t(0)
+    vol._check(getattr(vol._lib, fn_name)(vol._h, dp(d_verts), int(nverts), dp(d_tris), int(ntris), *args,
+                                          dp(d_out_verts), dp(d_out_tris), C.byref(nv), C.byref(nt)))
+    return nv.value, nt.value
+
+
+def flattenVerticesDevice(vol: TSDFVolumeOctree, d_verts, nverts: int, d_tris, ntris: int, d_out_verts, d_out_tris,
+                          min_dist: float = 0.0001):
+    """flattenVertices (integrate.cpp:103-150) on device arrays -> (nverts, ntris) written to d_out_verts / d_out_tris"""
+    return _meshpost_device("b200tsdf_mesh_flatten_device", vol, d_verts, nverts, d_tris, ntris, d_out_verts, d_out_tris,
+                            C.c_float(min_dist))
+
+
+def cleanupMeshDevice(vol: TSDFVolumeOctree, d_verts, nverts: int, d_tris, ntris: int, d_out_verts, d_out_tris,
+                      face_dist: float = 0.02, min_neighbors: int = 5):
+    """cleanupMesh (integrate.cpp:152-214) on device arrays -> (nverts, ntris) written to d_out_verts / d_out_tris"""
+    return _meshpost_device("b200tsdf_mesh_cleanup_device", vol, d_verts, nverts, d_tris, ntris, d_out_verts, d_out_tris,
+                            C.c_float(face_dist), int(min_neighbors))

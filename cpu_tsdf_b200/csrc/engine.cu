@@ -814,12 +814,13 @@ int download (b200tsdf* h, const void* d, size_t bytes, void*& host)
 // The enumeration behind marching cubes and getLeaves, in the reference's depth-first order.  launch (emit, total, keys, v, c)
 // enqueues the caller's kernels: with emit = std::false_type they add their record count to *total, with std::true_type they
 // also write their records at the slots they reserve, with the order key of each in keys.  A record is `words` 32-bit words
-// in v, plus `words` bytes in c when host_c is given.  The records are counted, emitted into device buffers of exactly that
-// size, sorted by the low key_bits of their keys and copied into host_v / *host_c (see download).  A failed allocation
-// returns B200TSDF_ENOMEM.
-template <typename Launch>
-int sorted_records (b200tsdf* h, const char* what, int words, int key_bits, const Launch& launch,
-                    void*& host_v, void** host_c, unsigned long long& count)
+// in v, plus `words` bytes in c.  The records are counted; then dest (count, v_out, c_out) names the device buffers that
+// receive them (v_out: count * words words; c_out: count * words bytes, or null for no colour bytes), or leaves v_out null
+// to stop after the count, or returns an error.  Otherwise the records are emitted into device buffers of exactly that size
+// and sorted by the low key_bits of their keys straight into v_out / c_out.  A failed allocation returns B200TSDF_ENOMEM.
+template <typename Launch, typename Dest>
+int sorted_records (b200tsdf* h, const char* what, int words, int key_bits, const Launch& launch, const Dest& dest,
+                    unsigned long long& count)
 {
   cudaStream_t s = h->stream;
   unsigned long long* d_total = h->d_stats + ST_SCRATCH;
@@ -828,19 +829,38 @@ int sorted_records (b200tsdf* h, const char* what, int words, int key_bits, cons
   launch (std::false_type (), d_total, nullptr, nullptr, nullptr);
   CK (cudaMemcpyAsync (&count, d_total, sizeof (count), cudaMemcpyDeviceToHost, s));
   CK (cudaStreamSynchronize (s));
-  const size_t nw = (size_t) count * words, nc = host_c ? nw : 0;
-  DevBuf<uint32_t> v (s), v2 (s); DevBuf<unsigned char> c (s), c2 (s); DevBuf<unsigned long long> k (s);
-  if (count)
+  void* v_out = nullptr; unsigned char* c_out = nullptr;
+  if (int rc = dest (count, v_out, c_out)) return rc;
+  if (!count || !v_out) return B200TSDF_OK;
+  const size_t nw = (size_t) count * words, nc = c_out ? nw : 0;
+  DevBuf<uint32_t> v (s); DevBuf<unsigned char> c (s); DevBuf<unsigned long long> k (s);
+  if (v.alloc (nw) || c.alloc (nc) || k.alloc (count)) return alloc_failed (h, what);
+  CK (cudaMemsetAsync (d_total, 0, sizeof (count), s));
+  launch (std::true_type (), d_total, k, v, c);
+  const int e = b2_sort_records (s, (size_t) count, key_bits, k, words, v, c, v_out, c_out);
+  if (e == (int) cudaErrorMemoryAllocation) return alloc_failed (h, std::string (what) + " sort");
+  if (e) return h->fail (B200TSDF_ECUDA, std::string (what) + " sort: " + cudaGetErrorString ((cudaError_t) e));
+  return B200TSDF_OK;
+}
+
+// sorted_records into library-owned host memory: the records are sorted into device buffers of their exact size and copied
+// into host_v / *host_c (see download; host_c == null: no colour bytes)
+template <typename Launch>
+int sorted_records_host (b200tsdf* h, const char* what, int words, int key_bits, const Launch& launch,
+                         void*& host_v, void** host_c, unsigned long long& count)
+{
+  DevBuf<uint32_t> v2 (h->stream); DevBuf<unsigned char> c2 (h->stream);
+  auto dest = [&] (unsigned long long n, void*& v_out, unsigned char*& c_out)
   {
-    if (v.alloc (nw) || v2.alloc (nw) || c.alloc (nc) || c2.alloc (nc) || k.alloc (count)) return alloc_failed (h, what);
-    CK (cudaMemsetAsync (d_total, 0, sizeof (count), s));
-    launch (std::true_type (), d_total, k, v, c);
-    const int e = b2_sort_records (s, (size_t) count, key_bits, k, words, v, c, v2, c2);
-    if (e == (int) cudaErrorMemoryAllocation) return alloc_failed (h, std::string (what) + " sort");
-    if (e) return h->fail (B200TSDF_ECUDA, std::string (what) + " sort: " + cudaGetErrorString ((cudaError_t) e));
-  }
+    if (!n) return (int) B200TSDF_OK;
+    if (v2.alloc ((size_t) n * words) || (host_c && c2.alloc ((size_t) n * words))) return alloc_failed (h, what);
+    v_out = v2; c_out = c2;
+    return (int) B200TSDF_OK;
+  };
+  if (int rc = sorted_records (h, what, words, key_bits, launch, dest, count)) return rc;
+  const size_t nw = (size_t) count * words;
   if (int rc = download (h, v2, nw * 4, host_v)) return rc;
-  return host_c ? download (h, c2, nc, *host_c) : B200TSDF_OK;
+  return host_c ? download (h, c2, nw, *host_c) : B200TSDF_OK;
 }
 
 } // namespace
@@ -1847,10 +1867,15 @@ int b200tsdf_render (b200tsdf_t* h, const double* pose, int downsample, void* ou
   return B200TSDF_OK;
 }
 
+} // extern "C"
+
 // ---- marching cubes (marching_cubes_tsdf_octree.cpp:108-236) --------------------------------------------
-int b200tsdf_mesh (b200tsdf_t* h, float w_min, int color_mode, float** verts, uint8_t** rgb, size_t* nverts)
+// The one mesh path of b200tsdf_mesh and b200tsdf_mesh_device: the brick walk as count and emit launches, handed to
+// sort (launch), which runs them through sorted_records with the caller's destination.  A triangle is one record of 9
+// words (its three vertices) and 9 colour bytes, which is already the layout of the result.
+template <typename Sort>
+static int marching_cubes (b200tsdf* h, float w_min, int color_mode, const Sort& sort)
 {
-  if (!h || !verts || !nverts) return B200TSDF_EINVAL;
   if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "reconstruct before reset()");
   cudaSetDevice (h->device);
   const Params& p = h->p;
@@ -1867,13 +1892,105 @@ int b200tsdf_mesh (b200tsdf_t* h, float w_min, int color_mode, float** verts, ui
     if (nb) k_mesh_bricks<E><<<bgrid, 128, 0, s>>> (p, mc, list, nb, total, (float*) v, c, keys);
     k_mesh_roots<E><<<rgrid, 128, 0, s>>> (p, mc, total, (float*) v, c, keys);
   };
+  if (int rc = sort (launch)) return rc;
+  return check_device_err (h);
+}
+
+extern "C" {
+
+int b200tsdf_mesh (b200tsdf_t* h, float w_min, int color_mode, float** verts, uint8_t** rgb, size_t* nverts)
+{
+  if (!h || !verts || !nverts) return B200TSDF_EINVAL;
   std::free (h->mesh_c); h->mesh_c = nullptr;
   unsigned long long ntri = 0;
-  if (int rc = sorted_records (h, "triangles", 9, 3 * p.L + 3, launch, h->mesh_v, color_mode ? &h->mesh_c : nullptr, ntri)) return rc;
+  const int key_bits = 3 * h->p.L + 3;
+  auto sort = [&] (const auto& launch)
+  { return sorted_records_host (h, "triangles", 9, key_bits, launch, h->mesh_v, color_mode ? &h->mesh_c : nullptr, ntri); };
+  if (int rc = marching_cubes (h, w_min, color_mode, sort)) return rc;
   *nverts = (size_t) ntri * 3;
   *verts = ntri ? (float*) h->mesh_v : nullptr;
   if (rgb) *rgb = ntri ? (uint8_t*) h->mesh_c : nullptr;
-  return check_device_err (h);
+  return B200TSDF_OK;
+}
+
+int b200tsdf_mesh_device (b200tsdf_t* h, float w_min, int color_mode, float* d_verts, uint8_t* d_rgb, size_t capacity,
+                          size_t* nverts)
+{
+  if (!h || !nverts) return B200TSDF_EINVAL;
+  *nverts = 0;
+  if ((uintptr_t) d_verts & 3) return h->fail (B200TSDF_EINVAL, "d_verts must be 4-byte aligned");
+  unsigned long long ntri = 0;
+  auto dest = [&] (unsigned long long n, void*& v_out, unsigned char*& c_out)
+  {
+    *nverts = (size_t) n * 3;
+    if (!d_verts) return (int) B200TSDF_OK;                                        // count only
+    if (capacity < *nverts)
+      return h->fail (B200TSDF_EINVAL, "capacity " + std::to_string (capacity) + " < " + std::to_string (*nverts) + " vertices");
+    v_out = d_verts; c_out = color_mode ? d_rgb : nullptr;
+    return (int) B200TSDF_OK;
+  };
+  auto sort = [&] (const auto& launch) { return sorted_records (h, "triangles", 9, 3 * h->p.L + 3, launch, dest, ntri); };
+  return marching_cubes (h, w_min, color_mode, sort);
+}
+
+} // extern "C"
+
+// ---- flattenVertices / cleanupMesh on device arrays (b2_mesh_flatten / b2_mesh_cleanup, meshpost.cu) ----------------------
+static bool overlaps (const void* a, size_t na, const void* b, size_t nb)
+{
+  const uintptr_t x = (uintptr_t) a, y = (uintptr_t) b;
+  return na && nb && x < y + nb && y < x + na;
+}
+
+// the checks that need no data; the routine checks the indices on the device
+static int meshpost_device_args (b200tsdf* h, const float* d_verts, size_t nverts, const int32_t* d_tris, size_t ntris,
+                                 const float* d_out_verts, const int32_t* d_out_tris, size_t* out_nverts, size_t* out_ntris)
+{
+  if (!out_nverts || !out_ntris) return h->fail (B200TSDF_EINVAL, "null argument");
+  *out_nverts = 0; *out_ntris = 0;
+  if ((!d_verts || !d_out_verts) && nverts) return h->fail (B200TSDF_EINVAL, "null vertex array");
+  if (!d_out_tris && ntris) return h->fail (B200TSDF_EINVAL, "null triangle array");
+  if (nverts >= (size_t) 1 << 31 || ntris >= ((size_t) 1 << 31) / 3) return h->fail (B200TSDF_EINVAL, "mesh too large for 32-bit indices");
+  if (!d_tris && nverts != 3 * ntris) return h->fail (B200TSDF_EINVAL, "a triangle soup (d_tris == NULL) needs nverts == 3 * ntris");
+  if (((uintptr_t) d_verts | (uintptr_t) d_tris | (uintptr_t) d_out_verts | (uintptr_t) d_out_tris) & 3)
+    return h->fail (B200TSDF_EINVAL, "device arrays must be 4-byte aligned");
+  const size_t bv = 12 * nverts, bt = 12 * ntris, bt_in = d_tris ? bt : 0;          // a soup has no triangle input
+  if (overlaps (d_out_verts, bv, d_verts, bv) || overlaps (d_out_verts, bv, d_tris, bt_in) || overlaps (d_out_verts, bv, d_out_tris, bt)
+      || overlaps (d_out_tris, bt, d_verts, bv) || overlaps (d_out_tris, bt, d_tris, bt_in))
+    return h->fail (B200TSDF_EINVAL, "outputs overlap the inputs or each other");
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "mesh post-processing before reset()");
+  cudaSetDevice (h->device);
+  return pending_device_err (h);
+}
+
+extern "C" {
+
+int b200tsdf_mesh_flatten_device (b200tsdf_t* h, const float* d_verts, size_t nverts, const int32_t* d_tris, size_t ntris,
+                                  float min_dist, float* d_out_verts, int32_t* d_out_tris, size_t* out_nverts, size_t* out_ntris)
+{
+  if (!h) return B200TSDF_EINVAL;
+  if (int rc = meshpost_device_args (h, d_verts, nverts, d_tris, ntris, d_out_verts, d_out_tris, out_nverts, out_ntris)) return rc;
+  B2MeshScratch scratch;
+  std::string err;
+  if (int rc = b2_mesh_flatten (h->stream, scratch, d_verts, nverts, d_tris, ntris, min_dist, d_out_verts, d_out_tris,
+                                out_nverts, out_ntris, err))
+    return h->fail (rc, "flattenVertices: " + err);
+  return B200TSDF_OK;
+}
+
+int b200tsdf_mesh_cleanup_device (b200tsdf_t* h, const float* d_verts, size_t nverts, const int32_t* d_tris, size_t ntris,
+                                  float face_dist, int min_neighbors,
+                                  float* d_out_verts, int32_t* d_out_tris, size_t* out_nverts, size_t* out_ntris)
+{
+  if (!h) return B200TSDF_EINVAL;
+  if (min_neighbors < 1 || min_neighbors > 16) return h->fail (B200TSDF_EINVAL, "min_neighbors must be in 1..16");
+  if (int rc = meshpost_device_args (h, d_verts, nverts, d_tris, ntris, d_out_verts, d_out_tris, out_nverts, out_ntris)) return rc;
+  B2MeshScratch scratch;
+  std::string err;
+  if (int rc = b2_mesh_cleanup (h->stream, scratch, d_verts, nverts, d_tris, ntris, face_dist, min_neighbors, d_out_verts, d_out_tris,
+                                out_nverts, out_ntris, err))
+    return h->fail (rc, "cleanupMesh: " + err);
+  return B200TSDF_OK;
 }
 
 void b200tsdf_free (void* p) { (void) p; /* mesh buffers are owned by the handle */ }
@@ -1954,7 +2071,7 @@ int enumerate_leaves (b200tsdf* h, int nlevels, bool occupied, const char* what,
       if (nb) k_leaves_bricks<E><<<bgrid, 128, 0, s>>> (p, list, nb, nlevels, occ, total, keys, (uint32_t*) rec);
       k_leaves_roots<E><<<rgrid, 128, 0, s>>> (p, nlevels, occ, total, keys, (uint32_t*) rec);
     };
-    if (int rc = sorted_records (h, "leaf records", 3, 3 * p.L, launch, out, nullptr, count)) return rc;
+    if (int rc = sorted_records_host (h, "leaf records", 3, 3 * p.L, launch, out, nullptr, count)) return rc;
   }
   h->d2h_bytes += (long long) (count * 12);
   *n = (size_t) count;

@@ -187,6 +187,16 @@ int  b200tsdf_render_batch_device (b200tsdf_t* h, int n, const double* poses_c2w
  * b200tsdf_free.  B200TSDF_ENOMEM when the triangle or sort buffers do not fit. */
 int  b200tsdf_mesh (b200tsdf_t* h, float w_min, int color_mode, float** verts, uint8_t** rgb, size_t* nverts);
 void b200tsdf_free (void* p);
+/* b200tsdf_mesh into device memory of h's device: the same vertices and colours, in the same order.  d_verts: 3 floats per
+ * vertex (4-byte aligned); d_rgb: 3 bytes per vertex, or NULL.  capacity: vertices d_verts can hold.  *nverts receives the
+ * vertex count (3 per triangle) once the volume has been walked.  d_verts == NULL: count only, nothing is written.
+ * capacity < count: B200TSDF_EINVAL, nothing is written.  Exactly 12 * count bytes of d_verts and, when color_mode != 0 and
+ * d_rgb != NULL, 3 * count bytes of d_rgb are written.  Ordered after every integrate queued on the handle; returns once the
+ * mesh is written (the handle's stream is synchronised, since the count has to reach the host).  Buffers the caller used on
+ * its own stream must be idle before the call.  B200TSDF_ESTATE before reset(), B200TSDF_ENOMEM when the triangle or sort
+ * buffers do not fit. */
+int  b200tsdf_mesh_device (b200tsdf_t* h, float w_min, int color_mode, float* d_verts, uint8_t* d_rgb, size_t capacity,
+                           size_t* nverts);
 
 /* ---- mesh post-processing of the reference's `integrate` program (no volume handle needed) ----------
  * Meshes are indexed: nverts xyz triples + ntris index triples (a marching-cubes soup is tris = 0,1,2,...).
@@ -197,12 +207,29 @@ void b200tsdf_free (void* p);
 int  b200tsdf_mesh_flatten (int device, const float* verts, size_t nverts, const int32_t* tris, size_t ntris, float min_dist,
                             float** out_verts, size_t* out_nverts, int32_t** out_tris, size_t* out_ntris);
 /* cleanupMesh (src/prog/integrate.cpp:152-214): faces whose centroids form clusters (cluster tolerance
- * face_dist) of at most min_neighbors faces are removed, then the vertices no face uses. */
+ * face_dist) of at most min_neighbors faces are removed, then the vertices no face uses.
+ * Both check the triangle indices on the device (the routine of b200tsdf_mesh_flatten_device / _cleanup_device below), so
+ * the mesh is uploaded before a bad index is refused with B200TSDF_EINVAL, and without a CUDA device that call fails with
+ * B200TSDF_ENODEVICE first. */
 int  b200tsdf_mesh_cleanup (int device, const float* verts, size_t nverts, const int32_t* tris, size_t ntris,
                             float face_dist, int min_neighbors,
                             float** out_verts, size_t* out_nverts, int32_t** out_tris, size_t* out_ntris);
 void b200tsdf_mesh_free (void* p);
 const char* b200tsdf_meshpost_last_error (void);   /* thread-local message of the last failed call above */
+/* b200tsdf_mesh_flatten / _cleanup on arrays in device memory of h's device, on h's stream, with the same result bit for bit.
+ * d_tris == NULL: a triangle soup, triangle t = {3t, 3t+1, 3t+2}, and nverts must equal 3 * ntris (no index array is
+ * built).  The outputs are the caller's and sized like the inputs: d_out_verts 3 * nverts floats, d_out_tris 3 * ntris int32
+ * (all four arrays 4-byte aligned); a result never exceeds its input and no byte past *out_nverts / *out_ntris entries is
+ * written.  The outputs must not overlap the inputs or each other; the inputs are only read.  The indices are checked on
+ * the device: one out of range gives B200TSDF_EINVAL before any output byte is written.  Limits as for the host entry
+ * points (nverts < 2^31, min_neighbors in 1..16); B200TSDF_ESTATE before reset(), B200TSDF_ENOMEM when the scratch does not
+ * fit; a pending device error of an earlier frame is reported as by the other reads.  Returns once the outputs are written.
+ * Errors come through b200tsdf_last_error (h). */
+int  b200tsdf_mesh_flatten_device (b200tsdf_t* h, const float* d_verts, size_t nverts, const int32_t* d_tris, size_t ntris,
+                                   float min_dist, float* d_out_verts, int32_t* d_out_tris, size_t* out_nverts, size_t* out_ntris);
+int  b200tsdf_mesh_cleanup_device (b200tsdf_t* h, const float* d_verts, size_t nverts, const int32_t* d_tris, size_t ntris,
+                                   float face_dist, int min_neighbors,
+                                   float* d_out_verts, int32_t* d_out_tris, size_t* out_nverts, size_t* out_ntris);
 
 /* Diagnostics: per-phase timing of the bottom-up per-cell kernel (k_celltop_up).  The first call arms the counters,
  * every call returns and clears them: out16[0..5] = max SM cycles << 32 | tag (total, level-3, level-2, level-1, cell,
