@@ -80,7 +80,21 @@ EXPORTS = [
     "b200tsdf_profile_begin", "b200tsdf_profile_end",
     "b200tsdf_mesh_flatten", "b200tsdf_mesh_cleanup", "b200tsdf_mesh_free", "b200tsdf_meshpost_last_error", "b200tsdf_debug_timing",
     "b200tsdf_mesh_device", "b200tsdf_mesh_flatten_device", "b200tsdf_mesh_cleanup_device",
+    "b200tsdf_containing_voxels", "b200tsdf_containing_voxels_device", "b200tsdf_dense_device",
 ]
+
+# b200tsdf_voxel (include/b200tsdf.h): one record of getContainingVoxel; level -1 = NULL
+VOXEL_DTYPE = np.dtype([("level", "<i4"), ("x", "<i4"), ("y", "<i4"), ("z", "<i4"),
+                        ("cx", "<f4"), ("cy", "<f4"), ("cz", "<f4"), ("size", "<f4"),
+                        ("d", "<f4"), ("w", "<f4"), ("r", "u1"), ("g", "u1"), ("b", "u1"), ("has_children", "u1")])
+
+
+class Voxel(C.Structure):
+    """b200tsdf_voxel (include/b200tsdf.h)"""
+    _fields_ = [("level", C.c_int32), ("x", C.c_int32), ("y", C.c_int32), ("z", C.c_int32),
+                ("cx", C.c_float), ("cy", C.c_float), ("cz", C.c_float), ("size", C.c_float),
+                ("d", C.c_float), ("w", C.c_float), ("r", C.c_uint8), ("g", C.c_uint8), ("b", C.c_uint8),
+                ("has_children", C.c_uint8)]
 
 _lib = None
 
@@ -141,6 +155,9 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_voxel_centers.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(C.c_size_t)]
     lib.b200tsdf_occupied_voxel_indices.argtypes = [vp, C.POINTER(vp), C.POINTER(C.c_size_t)]
     lib.b200tsdf_is_empty.argtypes = [vp, C.POINTER(C.c_int32)]
+    lib.b200tsdf_containing_voxels.argtypes = [vp, vp, C.c_size_t, C.c_float, vp]
+    lib.b200tsdf_containing_voxels_device.argtypes = [vp, vp, C.c_size_t, C.c_float, vp]
+    lib.b200tsdf_dense_device.argtypes = [vp, C.POINTER(C.c_int32), vp, vp, vp, vp]
     lib.b200tsdf_get_stats.argtypes = [vp, C.POINTER(Stats)]
     lib.b200tsdf_download_nodes.argtypes = [vp, vp, vp, vp, vp, vp, vp]; lib.b200tsdf_download_nodes.restype = C.c_int64
     lib.b200tsdf_download_color_payload.argtypes = [vp, vp]; lib.b200tsdf_download_color_payload.restype = C.c_int64
@@ -531,6 +548,31 @@ class TSDFVolumeOctree:
         buf, n = C.c_void_p(), C.c_size_t()
         self._check(self._lib.b200tsdf_occupied_voxel_indices(self._h, C.byref(buf), C.byref(n)))
         return self._leaf_records(buf, n.value, np.int32)
+
+    def getContainingVoxels(self, pts, min_size: float = -1.0) -> np.ndarray:
+        """octree_->getContainingVoxel (x, y, z, min_size) (octree.cpp:112-121, 628-634) at every point, with the node's
+        getCenter / getSize / getData / getRGB / hasChildren: a structured array of VOXEL_DTYPE, level -1 where the reference
+        returns NULL."""
+        xyz = np.ascontiguousarray(pts, dtype=np.float32).reshape(-1, 3)
+        out = np.zeros(len(xyz), VOXEL_DTYPE)
+        self._check(self._lib.b200tsdf_containing_voxels(self._h, _ptr(xyz), len(xyz), float(min_size), _ptr(out)))
+        return out
+
+    def getContainingVoxelsDevice(self, d_xyz: int, n: int, d_out: int, min_size: float = -1.0) -> bool:
+        """getContainingVoxels at n device points (3 floats each) into n 44-byte b200tsdf_voxel records at d_out"""
+        dp = lambda a: None if a is None else C.c_void_p(int(a))
+        self._check(self._lib.b200tsdf_containing_voxels_device(self._h, dp(d_xyz), int(n), float(min_size), dp(d_out)))
+        return True
+
+    def extractDenseDevice(self, box, d_d: int | None = None, d_w: int | None = None, d_rgb: int | None = None,
+                           d_level: int | None = None) -> bool:
+        """the point lookup at getVoxelCenter (i, j, k) for every finest voxel of box = (i0, j0, k0, i1, j1, k1), written as
+        C-contiguous [i1-i0, j1-j0, k1-k0] device arrays: d_d / d_w float32, d_rgb uint8 [.., 3], d_level int8 (the node's
+        depth).  An output left as None is not written."""
+        b = (C.c_int32 * 6)(*[int(v) for v in box])
+        dp = lambda a: None if a is None else C.c_void_p(int(a))
+        self._check(self._lib.b200tsdf_dense_device(self._h, b, dp(d_d), dp(d_w), dp(d_rgb), dp(d_level)))
+        return True
 
     def isEmpty(self) -> bool:
         """tsdf_volume_octree.h:283-287 — True after reset(), False after any integrateCloud, the file's flag after load()."""

@@ -286,6 +286,48 @@ __global__ void k_interpolate (Params gp, const float* __restrict__ xyz, int n, 
   valid[i] = v ? 1 : 0;
 }
 
+// Octree::getContainingVoxel (x, y, z, min_size) and the node's accessors, one thread per point
+__global__ void k_voxels (Params gp, const float* __restrict__ xyz, size_t n, float min_size, VoxelRec* __restrict__ out)
+{
+  B2_STAGE_PARAMS (gp)
+  const size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  out[i] = find_voxel (p, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], min_size);
+}
+
+// Dense crop of the box [i0, i1) x [j0, j1) x [k0, k1): one CTA per 8x8x8 tile (the finest voxels of one level L-3 node),
+// clipped to the box.  Thread 0 walks the tile's path once (dense_tile_walk); every voxel then resolves its leaf from the
+// tier-0 brick's split words, staged with the path in shared memory.  Outputs are [i][j][k], k fastest: eight consecutive
+// threads write one run along k.
+struct DenseBox { int i0, j0, k0, i1, j1, k1; int ti0, tj0, tk0, ntj, ntk; };
+constexpr int DENSE_THREADS = 256;
+
+__global__ void __launch_bounds__ (DENSE_THREADS) k_dense (Params gp, DenseBox b, float* __restrict__ d_d, float* __restrict__ d_w,
+                                                           unsigned char* __restrict__ d_rgb, signed char* __restrict__ d_level)
+{
+  __shared__ DenseTile st;
+  B2_STAGE_PARAMS (gp)
+  const unsigned tile = blockIdx.x;
+  const int tz = b.tk0 + (int) (tile % (unsigned) b.ntk);
+  const int ty = b.tj0 + (int) ((tile / (unsigned) b.ntk) % (unsigned) b.ntj);
+  const int tx = b.ti0 + (int) (tile / ((unsigned) b.ntk * (unsigned) b.ntj));
+  if (threadIdx.x == 0) dense_tile_walk (p, tx, ty, tz, st);
+  __syncthreads ();
+  const size_t nj = (size_t) (b.j1 - b.j0), nk = (size_t) (b.k1 - b.k0);
+  for (int v = threadIdx.x; v < 512; v += DENSE_THREADS)
+  {
+    const int X = 8 * tx + (v >> 6), Y = 8 * ty + ((v >> 3) & 7), Z = 8 * tz + (v & 7);
+    if (X < b.i0 || X >= b.i1 || Y < b.j0 || Y >= b.j1 || Z < b.k0 || Z >= b.k1) continue;
+    float2 dw; uchar4 c; int level;
+    dense_voxel (p, st, X, Y, Z, dw, c, level);
+    const size_t o = ((size_t) (X - b.i0) * nj + (size_t) (Y - b.j0)) * nk + (size_t) (Z - b.k0);
+    if (d_d) d_d[o] = dw.x;
+    if (d_w) d_w[o] = dw.y;
+    if (d_rgb) { d_rgb[3 * o] = c.x; d_rgb[3 * o + 1] = c.y; d_rgb[3 * o + 2] = c.z; }
+    if (d_level) d_level[o] = (signed char) level;
+  }
+}
+
 // renderView for a batch of poses: blockIdx.z is the pose within the launch, and each block stages that pose's record.  Pixels
 // are row-major, one image after the other; each gets 12 bytes of xyz at xyz_off and 12 of normal at normal_off (4-byte
 // aligned), and no other byte of the caller's buffer is written.  rgb: 3 bytes per pixel, or null.
@@ -1781,6 +1823,81 @@ int b200tsdf_interpolate (b200tsdf_t* h, const float* xyz, int n, float* val, ui
   note_device_err (h, s);
   CK (cudaStreamSynchronize (s));
   return pending_device_err (h);
+}
+
+// ---- octree_->getContainingVoxel and dense crops (octree.cpp:112-121, 628-643; tsdf_volume_octree.cpp:553-560) -------------
+static_assert (sizeof (VoxelRec) == sizeof (b200tsdf_voxel) && sizeof (b200tsdf_voxel) == 44, "b200tsdf_voxel layout");
+
+static int voxel_read_state (b200tsdf* h, const char* what)
+{
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, std::string (what) + " before reset()");
+  if (h->p.shard_count > 1)
+    return h->fail (B200TSDF_ESTATE, std::string (what) + " on a shard: a shard keeps the coarse cells it does not own as unsplit leaves; "
+                    "read the replica built by b200tsdf_gather_volume");
+  return B200TSDF_OK;
+}
+
+static bool aligned4 (const void* a) { return ((uintptr_t) a & 3u) == 0; }
+
+int b200tsdf_containing_voxels_device (b200tsdf_t* h, const float* d_xyz, size_t n, float min_size, b200tsdf_voxel* d_out)
+{
+  if (!h) return B200TSDF_EINVAL;
+  if (int rc = voxel_read_state (h, "getContainingVoxel")) return rc;
+  if (n == 0) return B200TSDF_OK;
+  if (!d_xyz || !d_out) return h->fail (B200TSDF_EINVAL, "missing point or output buffer");
+  if (!aligned4 (d_xyz) || !aligned4 (d_out)) return h->fail (B200TSDF_EINVAL, "point and output buffers must be 4-byte aligned");
+  if (n > ((size_t) INT_MAX) * 128) return h->fail (B200TSDF_EINVAL, "too many points for one call");
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  k_voxels<<<(unsigned) ((n + 127) / 128), 128, 0, h->stream>>> (h->p, d_xyz, n, min_size, reinterpret_cast<VoxelRec*> (d_out));
+  CK (cudaGetLastError ());
+  note_device_err (h, h->stream);
+  return B200TSDF_OK;
+}
+
+int b200tsdf_containing_voxels (b200tsdf_t* h, const float* xyz, size_t n, float min_size, b200tsdf_voxel* out)
+{
+  if (!h) return B200TSDF_EINVAL;
+  if (int rc = voxel_read_state (h, "getContainingVoxel")) return rc;
+  if (n == 0) return B200TSDF_OK;
+  if (!xyz || !out) return h->fail (B200TSDF_EINVAL, "missing point or output buffer");
+  cudaSetDevice (h->device);
+  // one scratch block: xyz (12 n) | records (44 n)
+  { int rc = h->scratch (n * (12 + sizeof (b200tsdf_voxel)) + 64); if (rc) return rc; }
+  float* d_xyz = (float*) h->d_scratch;
+  b200tsdf_voxel* d_out = (b200tsdf_voxel*) (d_xyz + 3 * n);
+  cudaStream_t s = h->stream;
+  CK (cudaMemcpyAsync (d_xyz, xyz, n * 12, cudaMemcpyHostToDevice, s));
+  if (int rc = b200tsdf_containing_voxels_device (h, d_xyz, n, min_size, d_out)) return rc;
+  CK (cudaMemcpyAsync (out, d_out, n * sizeof (b200tsdf_voxel), cudaMemcpyDeviceToHost, s));
+  note_device_err (h, s);
+  CK (cudaStreamSynchronize (s));
+  return pending_device_err (h);
+}
+
+int b200tsdf_dense_device (b200tsdf_t* h, const int32_t box[6], float* d_d, float* d_w, uint8_t* d_rgb, int8_t* d_level)
+{
+  if (!h) return B200TSDF_EINVAL;
+  if (int rc = voxel_read_state (h, "dense crop")) return rc;
+  if (!box) return h->fail (B200TSDF_EINVAL, "missing box");
+  if (!d_d && !d_w && !d_rgb && !d_level) return h->fail (B200TSDF_EINVAL, "no output buffer");
+  for (int a = 0; a < 3; ++a)
+    if (!(0 <= box[a] && box[a] < box[a + 3] && box[a + 3] <= h->p.res))
+      return h->fail (B200TSDF_EINVAL, "box must satisfy 0 <= lo < hi <= resolution on every axis");
+  if (!aligned4 (d_d) || !aligned4 (d_w)) return h->fail (B200TSDF_EINVAL, "d_d and d_w must be 4-byte aligned");
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  DenseBox b;
+  b.i0 = box[0]; b.j0 = box[1]; b.k0 = box[2]; b.i1 = box[3]; b.j1 = box[4]; b.k1 = box[5];
+  b.ti0 = b.i0 >> 3; b.tj0 = b.j0 >> 3; b.tk0 = b.k0 >> 3;
+  const int nti = ((b.i1 - 1) >> 3) - b.ti0 + 1;
+  b.ntj = ((b.j1 - 1) >> 3) - b.tj0 + 1; b.ntk = ((b.k1 - 1) >> 3) - b.tk0 + 1;
+  const unsigned long long tiles = (unsigned long long) nti * b.ntj * b.ntk;      // one CTA per tile: 2^27 for a whole 4096^3 grid
+  if (tiles > (unsigned long long) INT_MAX) return h->fail (B200TSDF_EINVAL, "box too large for one call (more than 2^31 - 1 tiles of 8^3)");
+  k_dense<<<(unsigned) tiles, DENSE_THREADS, 0, h->stream>>> (h->p, b, d_d, d_w, d_rgb, (signed char*) d_level);
+  CK (cudaGetLastError ());
+  note_device_err (h, h->stream);
+  return B200TSDF_OK;
 }
 
 // ---- renderView / renderColoredView (tsdf_volume_octree.cpp:278-450) ----------------------------------

@@ -924,6 +924,117 @@ B2_HD Leaf find_leaf (const Params& p, float x, float y, float z) { Leaf l; find
 B2_HD Leaf find_leaf (const Params& p, float x, float y, float z) { return find_leaf_impl (p, x, y, z); }
 #endif
 
+// ---- Octree::getContainingVoxel (x, y, z, min_size) and the node's accessors (octree.cpp:52-142, 173-178, 628-643) ----
+// One record per lookup, the layout of b200tsdf_voxel (include/b200tsdf.h).  level -1: the reference returns NULL.
+struct VoxelRec
+{
+  int level, x, y, z;
+  float cx, cy, cz, size;       // getCenter / getSize
+  float d, w;                   // getData
+  unsigned char r, g, b;        // getRGB
+  unsigned char has_children;   // hasChildren
+};
+
+// the record of node n.  Nodes above the root arrays and the virtual levels above the coarse depth carry no state: they
+// report the constructor's (d = -1, w = 0, the colour of a fresh node).
+B2_HD VoxelRec voxel_record (const Params& p, const NodePos& n, bool has_children)
+{
+  VoxelRec o;
+  o.level = n.level; o.x = n.x; o.y = n.y; o.z = n.z;
+  o.cx = n.cx; o.cy = n.cy; o.cz = n.cz; o.size = n.size;
+  const bool stored = n.level >= p.Rtop && n.level >= p.C;
+  const float2 dw = stored ? *node_dw (p, n) : make_float2 (-1.f, 0.f);
+  o.d = dw.x; o.w = dw.y;
+  if (!p.color) o.r = o.g = o.b = 127;                     // OctreeNode::getRGB, octree.cpp:173-178
+  else if (!stored) o.r = o.g = o.b = 0;                   // RGBNode / RGBNormalized constructors (octree.h:177, :217-223)
+  else { const uchar4 c = node_get_rgb (p, n); o.r = c.x; o.g = c.y; o.b = c.z; }
+  o.has_children = has_children ? 1 : 0;
+  return o;
+}
+
+// Octree::getContainingVoxel (octree.cpp:628-634) then OctreeNode::getContainingVoxel (:112-121): descend with the strict
+// (x - ctr) > 0 per axis and stop at a leaf or at the first node with min_size > 0 && size_ <= min_size.
+B2_HD VoxelRec find_voxel (const Params& p, float x, float y, float z, float min_size)
+{
+  if (is_nan (z) || fabsf (x) > p.half || fabsf (y) > p.half || fabsf (z) > p.half)
+  {
+    VoxelRec o = {};
+    o.level = -1;
+    return o;
+  }
+  NodePos n;
+  n.level = 0; n.x = n.y = n.z = 0; n.cx = n.cy = n.cz = 0.f; n.size = p.size; n.slot = -1; n.idx = 0;
+  for (;;)
+  {
+    const bool split = n.level < p.Rtop || is_split (p, n);            // levels above the root arrays are split by init
+    if (!split || (min_size > 0.f && n.size <= min_size)) return voxel_record (p, n, split);
+    const int cs = n.level < p.Rtop ? -1 : children_slot (p, n, false);
+    if (n.level >= p.Rtop && cs < 0) return voxel_record (p, n, split);   // cannot happen when the invariant holds
+    const int c = ((fsub (x, n.cx) > 0) << 2) | ((fsub (y, n.cy) > 0) << 1) | (int) (fsub (z, n.cz) > 0);
+    n = make_child (p, n, c, cs);
+    if (n.level == p.Rtop) n.idx = root_index (p, n.x, n.y, n.z);
+  }
+}
+
+// ---- dense crop: the point lookup at every voxel centre of a box, one 8x8x8 tile at a time -------------------------------
+// A tile is the finest-level box of one level L-3 node (a tier-0 brick root).  The tile's path is walked once by index — root
+// array, split bits, one find_brick per tier — and each voxel's leaf is then resolved inside the tier-0 brick from the three
+// bits of its brick-local coordinates.  The index descent equals the float descent at the voxel centres (DESIGN.md §3c).
+// reset() refuses L <= C, so T >= 1 and L - 3 >= Rtop on every grid: the smallest ones (8^3 over a coarse depth of 0..2) are
+// one tile whose path starts and ends at the root arrays.
+struct DenseTile
+{
+  int mode;                     // 0: node `n` (a leaf at level <= L-3) covers the tile; 1: tier-0 brick `slot` below node `n`
+  int slot;
+  NodePos n;
+  uint32_t sw[BRICK_SPLIT_WORDS];
+};
+
+// tile (tx, ty, tz): finest voxels [8 tx, 8 tx + 8) x [8 ty, 8 ty + 8) x [8 tz, 8 tz + 8)
+B2_HD void dense_tile_walk (const Params& p, int tx, int ty, int tz, DenseTile& t)
+{
+  t.slot = -1;
+  const int TL = p.L - 3;
+  NodePos n = make_root (p, tx >> (TL - p.Rtop), ty >> (TL - p.Rtop), tz >> (TL - p.Rtop));
+  for (;;)
+  {
+    if (!is_split (p, n)) { t.mode = 0; t.n = n; return; }
+    const int cs = children_slot (p, n, false);
+    if (cs < 0) { t.mode = 0; t.n = n; return; }                        // cannot happen when the invariant holds
+    if (n.level == TL) { t.slot = cs; break; }
+    const int sh = TL - n.level - 1;
+    n = make_child (p, n, (((tx >> sh) & 1) << 2) | (((ty >> sh) & 1) << 1) | ((tz >> sh) & 1), cs);
+  }
+  t.mode = 1; t.n = n;
+  for (int i = 0; i < BRICK_SPLIT_WORDS; ++i) t.sw[i] = p.split[(size_t) t.slot * BRICK_SPLIT_WORDS + i];
+}
+
+// the leaf of finest voxel (X, Y, Z) of the tile: its storage and level
+B2_HD void dense_voxel (const Params& p, const DenseTile& t, int X, int Y, int Z, float2& dw, uchar4& c, int& level)
+{
+  NodePos n;
+  if (t.mode == 0) { n = t.n; }
+  else
+  {
+    n.slot = t.slot;
+    int k = 1;
+    for (;; ++k)
+    {
+      const int sh = 3 - k;
+      const int j = path_index (k, (X & 7) >> sh, (Y & 7) >> sh, (Z & 7) >> sh);
+      n.idx = node_offset (k) + j;
+      n.level = p.L - 3 + k;
+      if (k == 3) break;
+      const bool split = n.level < p.C || ((t.sw[split_word_base (k) + (j >> 5)] >> (j & 31)) & 1u);
+      if (!split) break;
+    }
+  }
+  level = n.level;
+  dw = *node_dw (p, n);
+  if (!p.color) c = make_uchar4 (127, 127, 127, 0);
+  else c = node_get_rgb (p, n);
+}
+
 // ---- getVoxelCenter / getVoxelIndex (tsdf_volume_octree.cpp:553-574) ----------------------------
 B2_HD float voxel_center1 (const Params& p, long long i)
 { return (float) (dadd (ddiv (dmul ((double) i + 0.5, p.dsize), p.dres), -(double) p.voff)); }

@@ -295,6 +295,40 @@ int  b200tsdf_occupied_voxel_indices (b200tsdf_t* h, int32_t** ijk, size_t* n);
  * value after b200tsdf_load.  B200TSDF_ESTATE before reset(). */
 int  b200tsdf_is_empty (b200tsdf_t* h, int32_t* out);
 
+/* ---- raw node reads: tsdf->octree_->getContainingVoxel (x, y, z, min_size) and the node's accessors ----
+ * Octree::getContainingVoxel (octree.cpp:628-634): NaN z, or |coordinate| > size/2 on any axis, gives NULL (level -1, every
+ * other field 0).  NaN x or y with a finite z descends with every comparison false, as in the reference.
+ * OctreeNode::getContainingVoxel (octree.cpp:112-121): the child is chosen with the strict (x - ctr) > 0 per axis (a point on
+ * a splitting plane goes to the lower child); the descent stops at a leaf or at the first node with
+ * min_size > 0 && size <= min_size, which may have children.  Nodes with no state of their own (above the root arrays, and
+ * the levels above the coarse depth, which Octree::init splits and nothing updates) report the constructor's state. */
+typedef struct b200tsdf_voxel
+{
+  int32_t level;              /* depth of the node, 0 = root; -1 when getContainingVoxel returns NULL (other fields then 0) */
+  int32_t x, y, z;            /* node index at its level                                                           */
+  float   cx, cy, cz, size;   /* OctreeNode::getCenter / getSize (octree.cpp:52-66)                                */
+  float   d, w;               /* OctreeNode::getData (octree.cpp:124-130)                                          */
+  uint8_t r, g, b;            /* getRGB: the stored bytes (RGBNode), the RGBNormalized conversion (octree.cpp:396-402),
+                                 127,127,127 without colour (OctreeNode::getRGB, octree.cpp:173-178)                */
+  uint8_t has_children;       /* OctreeNode::hasChildren (octree.cpp:41-45)                                        */
+} b200tsdf_voxel;             /* 44 bytes */
+
+/* n point lookups.  xyz: 3 floats per point, out: n records; host pointers (copied in, b200tsdf_containing_voxels_device,
+ * copied out).  B200TSDF_ESTATE before reset() and on a sharded handle (shard_count > 1: read the replica of
+ * b200tsdf_gather_volume); n == 0 is a no-op. */
+int  b200tsdf_containing_voxels (b200tsdf_t* h, const float* xyz, size_t n, float min_size, b200tsdf_voxel* out);
+/* the same on device memory of h's device (d_xyz and d_out 4-byte aligned).  Asynchronous on the handle's stream and ordered
+ * after every integrate queued on the handle; errors as for b200tsdf_query_device. */
+int  b200tsdf_containing_voxels_device (b200tsdf_t* h, const float* d_xyz, size_t n, float min_size, b200tsdf_voxel* d_out);
+/* Dense crop of the finest-voxel box [i0,i1) x [j0,j1) x [k0,k1) (box = {i0, j0, k0, i1, j1, k1}, host memory): entry (i,j,k)
+ * is the lookup with min_size = -1 at getVoxelCenter (i, j, k) (tsdf_volume_octree.cpp:553-560), written at offset
+ * ((i-i0)*(j1-j0) + (j-j0))*(k1-k0) + (k-k0) (64-bit: a whole 2048^3 box is 8.6 G entries).  d_d, d_w: getData (4-byte
+ * aligned floats); d_rgb: getRGB, 3 bytes per entry; d_level: the node's depth.  Any output may be NULL and is then not
+ * written; all four NULL is B200TSDF_EINVAL, as is a box without 0 <= lo < hi <= resolution on every axis.  No byte outside
+ * the box's extent is written.  Asynchronous, ordered and reported like b200tsdf_containing_voxels_device;
+ * B200TSDF_ESTATE before reset() and on a sharded handle. */
+int  b200tsdf_dense_device (b200tsdf_t* h, const int32_t box[6], float* d_d, float* d_w, uint8_t* d_rgb, int8_t* d_level);
+
 /* ---- introspection (tests, bench accounting) ------------------------------------------- */
 typedef struct b200tsdf_stats
 {

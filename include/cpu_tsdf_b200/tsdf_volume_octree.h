@@ -312,6 +312,38 @@ public:
     for (std::size_t i = 0; i < n; ++i) indices.push_back (detail::vector3i (v + 3 * i));
   }
 
+  // octree_->getContainingVoxel (x, y, z, min_size) (octree.cpp:112-121, 628-634): the node's state as a value.  Migration:
+  // `tsdf->octree_->getContainingVoxel (x, y, z)->getData (d, w)` becomes `tsdf->getContainingVoxel (x, y, z).getData (d, w)`;
+  // valid () is false where the reference returns NULL (or the call failed: see status ()).
+  struct Voxel
+  {
+    b200tsdf_voxel v;
+    bool valid () const { return v.level >= 0; }
+    void getCenter (float& x, float& y, float& z) const { x = v.cx; y = v.cy; z = v.cz; }
+    void getSize (float& sx, float& sy, float& sz) const { sx = sy = sz = v.size; }
+    float getMinSize () const { return v.size; }
+    bool getData (float& d, float& w) const { d = v.d; w = v.w; return true; }
+    bool getRGB (std::uint8_t& r, std::uint8_t& g, std::uint8_t& b) const { r = v.r; g = v.g; b = v.b; return true; }
+    bool hasChildren () const { return v.has_children != 0; }
+    int getDepth () const { return v.level; }
+  };
+  Voxel getContainingVoxel (float x, float y, float z, float min_size = -1) const
+  {
+    Voxel o{};
+    o.v.level = -1;
+    const float p[3] = { x, y, z };
+    status_ = h_ ? b200tsdf_containing_voxels (h_, p, 1, min_size, &o.v) : B200TSDF_ENODEVICE;
+    if (status_ != 0) { o.v = b200tsdf_voxel{}; o.v.level = -1; }
+    return o;
+  }
+  // the batch: xyz holds 3 floats per point; out receives one record per point (level -1 = NULL)
+  void getContainingVoxel (const std::vector<float>& xyz, std::vector<b200tsdf_voxel>& out, float min_size = -1) const
+  {
+    const std::size_t n = xyz.size () / 3;
+    out.assign (n, b200tsdf_voxel{});
+    status_ = h_ ? b200tsdf_containing_voxels (h_, xyz.data (), n, min_size, out.data ()) : B200TSDF_ENODEVICE;
+  }
+
   // h:283-287
   bool isEmpty () const
   {
