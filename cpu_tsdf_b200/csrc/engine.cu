@@ -1780,6 +1780,10 @@ int b200tsdf_query (b200tsdf_t* h, const float* xyz, int n, int what, int mode,
   unsigned char* d_ok = (unsigned char*) (d_hess + (size_t) 9 * n);
   cudaStream_t s = h->stream;
   CK (cudaMemcpyAsync (d_xyz, xyz, (size_t) n * 12, cudaMemcpyHostToDevice, s));
+  // the kernel writes the ok points only: the caller's values go in first, so that the rest come back as they were
+  if (what & 1) CK (cudaMemcpyAsync (d_val, val, (size_t) n * 4, cudaMemcpyHostToDevice, s));
+  if (what & 2) CK (cudaMemcpyAsync (d_grad, grad, (size_t) n * 12, cudaMemcpyHostToDevice, s));
+  if (what & 4) CK (cudaMemcpyAsync (d_hess, hess, (size_t) n * 36, cudaMemcpyHostToDevice, s));
   if (int rc = b200tsdf_query_device (h, d_xyz, n, what, mode, d_val, d_grad, d_hess, d_ok)) return rc;
   CK (cudaMemcpyAsync (ok, d_ok, (size_t) n, cudaMemcpyDeviceToHost, s));
   if (what & 1) CK (cudaMemcpyAsync (val, d_val, (size_t) n * 4, cudaMemcpyDeviceToHost, s));

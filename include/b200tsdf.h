@@ -149,8 +149,8 @@ int  b200tsdf_integrate_unorganized_batch_device (b200tsdf_t* h, int n, const vo
 
 /* getFxn / getGradient / getHessian (cpp:655-725) with mode 0, or the combined
  * getFxnAndGradient / getFxnGradientAndHessian (cpp:728-794) with mode 1.  what: bit0 value,
- * bit1 gradient (3 floats), bit2 hessian (9 floats, row-major).  ok[i] = the reference's bool.
- * xyz/val/grad/hess/ok are host pointers. */
+ * bit1 gradient (3 floats), bit2 hessian (9 floats, row-major).  ok[i] = the reference's bool; where it is 0 the outputs of
+ * point i keep the caller's values, as the reference leaves its reference arguments.  xyz/val/grad/hess/ok are host pointers. */
 int  b200tsdf_query (b200tsdf_t* h, const float* xyz, int n, int what, int mode,
                      float* val, float* grad, float* hess, uint8_t* ok);
 

@@ -182,10 +182,11 @@ class OracleVolume:
         return val, grad, hess, ok.astype(bool)
 
     def interpolate(self, xyz: np.ndarray, valid_in=True):
-        """getTSDFValue = interpolateTrilinearly (cpp:454-541).  Returns (values, valid) with valid starting as `valid_in`."""
+        """getTSDFValue = interpolateTrilinearly (cpp:454-541).  Returns (values, valid) with valid starting as `valid_in`
+        (one flag, or one per point)."""
         xyz = np.ascontiguousarray(xyz, dtype=np.float32).reshape(-1, 3)
         n = len(xyz)
-        val = np.zeros(n, np.float32); ok = np.full(n, 1 if valid_in else 0, np.uint8)
+        val = np.zeros(n, np.float32); ok = np.broadcast_to(np.asarray(valid_in, bool), (n,)).astype(np.uint8)
         self.lib.orc_interpolate(self.h, _ptr(xyz), n, _ptr(val), _ptr(ok))
         return val, ok.astype(bool)
 

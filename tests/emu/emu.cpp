@@ -214,6 +214,18 @@ int emu_query (const Emu* e, const float* xyz, int n, int what, int mode, float*
   return 0;
 }
 
+// k_interpolate: valid_in_out holds the caller's flags on entry and is only ever cleared
+int emu_interpolate (const Emu* e, const float* xyz, int n, float* val, uint8_t* valid_in_out)
+{
+  for (int i = 0; i < n; ++i)
+  {
+    bool v = valid_in_out[i] != 0;
+    val[i] = interpolate_trilinearly (e->p, xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], &v);
+    valid_in_out[i] = v ? 1 : 0;
+  }
+  return 0;
+}
+
 int emu_render (const Emu* e, const double* pose, int downsample, void* out, size_t stride, int xyz_off, int normal_off, uint8_t* rgb_out)
 {
   RenderParams r;

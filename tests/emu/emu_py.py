@@ -40,6 +40,7 @@ def load():
         lib.emu_stats.argtypes = [vp, vp]
         lib.emu_dump_nodes.argtypes = [vp] + [vp] * 6; lib.emu_dump_nodes.restype = C.c_longlong
         lib.emu_query.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
+        lib.emu_interpolate.argtypes = [vp, vp, C.c_int, vp, vp]
         lib.emu_render.argtypes = [vp, vp, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, vp]
         lib.emu_mesh.argtypes = [vp, C.c_float, C.c_int, C.POINTER(vp), C.POINTER(vp)]; lib.emu_mesh.restype = C.c_longlong
         lib.emu_levels.argtypes = [vp, vp]
@@ -127,6 +128,14 @@ class EmuVolume:
         hess = np.full((n, 3, 3), np.nan, np.float32); ok = np.zeros(n, np.uint8)
         self.lib.emu_query(self.h, _ptr(xyz), n, what, mode, _ptr(val), _ptr(grad), _ptr(hess), _ptr(ok))
         return val, grad, hess, ok.astype(bool)
+
+    def interpolate(self, xyz, valid_in=True):
+        """k_interpolate's routine; `valid_in` is one flag or one per point.  Returns (values, valid)."""
+        xyz = np.ascontiguousarray(xyz, dtype=np.float32).reshape(-1, 3)
+        n = len(xyz)
+        val = np.zeros(n, np.float32); ok = np.broadcast_to(np.asarray(valid_in, bool), (n,)).astype(np.uint8)
+        self.lib.emu_interpolate(self.h, _ptr(xyz), n, _ptr(val), _ptr(ok))
+        return val, ok.astype(bool)
 
     def render(self, pose, downsample=1, colored=False):
         W, H = self.cfg.image_width // downsample, self.cfg.image_height // downsample
