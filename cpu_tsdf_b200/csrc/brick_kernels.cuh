@@ -35,15 +35,54 @@ struct FrameRec
 {
   Frame f;
   float pl[6][4];          // frustum planes (host_math.h)
-  int cset;                // which of the two per-frame counter sets this frame uses
+  int cset;                // which of the two per-frame counter sets this frame uses; also selects the frame's pixel plane and cell queue
   int timing;              // 1: the brick kernel stamps kt[] with %globaltimer (profiling; works inside a replayed graph)
-  int pad_[2];
+  uint32_t seq;            // the frame's sequence number on its handle (the value of its fold marks, see FoldState)
+  int gated;               // 1: k_front waits per supercell for the previous frame's fold instead of for its whole last kernel
   unsigned long long kt[2];// [0] start of the brick kernel (ns), [1] end of its last block; zeroed by the record upload
 };
 // programmatic dependent launch: the hot kernels of a frame are launched with programmatic stream serialization, so the next
 // kernel's blocks become resident while this one drains and only wait (pdl_wait) before they touch what it wrote
 __device__ __forceinline__ void pdl_launch_dependents () { asm volatile ("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait () { asm volatile ("griddepcontrol.wait;" ::: "memory"); }
+
+// Per-supercell fold marks of the route whose supercells are the culled coarse cells (C == SL, no k_upper_* levels), over the
+// 8^C cells, all cleared by reset ():
+//   visited[s][c]  k_front's cull thread of a frame with counter set s stores the frame's seq when it queues cell c;
+//   folded[c]      k_celltop_up stores seq after its last write to cell c (every cell of its list, leaves included);
+//   opened         k_celltop_down stores seq once it has passed its griddepcontrol.wait: that frame's k_front is complete.
+// A gated k_front (FrameRec::gated) pre-splits a pixel of cell c as soon as the previous frame e-1 is done with c: after
+// `opened == e-1`, while `visited[s(e-1)][c] == e-1 && folded[c] != e-1` it waits.  The cull threads of frame e write
+// visited[s(e)], never the slot frame e's pixels read, so a pixel never sees its own frame's mark.
+struct FoldState
+{
+  uint32_t* visited;         // [2][ncells]
+  uint32_t* folded;          // [ncells]
+  uint32_t* opened;          // [1]
+};
+__host__ __device__ __forceinline__ FoldState fold_state (uint32_t* base, int C)
+{
+  const size_t n = (size_t) 1 << (3 * C);
+  FoldState s; s.visited = base; s.folded = base + 2 * n; s.opened = base + 3 * n;
+  return s;
+}
+__host__ __device__ __forceinline__ size_t fold_words (int C) { return 3 * ((size_t) 1 << (3 * C)) + 1; }
+__device__ __forceinline__ uint32_t ld_acquire (const uint32_t* a) { uint32_t v; asm volatile ("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(a) : "memory"); return v; }
+__device__ __forceinline__ uint32_t ld_relaxed (const uint32_t* a) { uint32_t v; asm volatile ("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(a) : "memory"); return v; }
+__device__ __forceinline__ void st_release (uint32_t* a, uint32_t v) { asm volatile ("st.release.gpu.global.u32 [%0], %1;" :: "l"(a), "r"(v) : "memory"); }
+// Spins until *a == want.  Bounded: the count is far beyond any fold (each round sleeps up to 1 us, so about 4 s of waiting),
+// after which ERR_FOLD_WAIT is raised and the caller goes on, so a broken protocol is an error of the next call, not a hang.
+constexpr int FOLD_SPIN_LIMIT = 1 << 22;
+__device__ __forceinline__ void wait_mark (const Params& p, const uint32_t* a, uint32_t want)
+{
+  unsigned ns = 32;
+  for (int it = 0; ld_acquire (a) != want; ++it)
+  {
+    if (it == FOLD_SPIN_LIMIT) { raise_err (p, ERR_FOLD_WAIT); return; }
+    __nanosleep (ns);
+    if (ns < 1024) ns <<= 1;
+  }
+}
 __device__ __forceinline__ unsigned long long global_ns () { unsigned long long t; asm volatile ("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
 constexpr int MAX_QLEVELS = 8;
@@ -460,11 +499,14 @@ __device__ __forceinline__ void top_kj (int f, int& k, int& j)
 //           is a supercell (static list, qslot < 0); the levels above C are virtual — they exist by Octree::init
 //           (octree.cpp:584-599), carry no state, are never observed, updated or pruned — and a node of level C is visited
 //           only when it passes the frustum cull and belongs to this shard (cpp:619-652), exactly like a queued coarse cell.
+//   cells / cells1: the supercell list of a frame with counter set 0 / 1 (the same list unless k_front fills it, see launch_frame);
+//   fold: the fold marks (FoldState) when this route publishes them, else null.
 template <bool COLOR>
-__global__ void __launch_bounds__ (TOP_THREADS) k_celltop_down (Params p, const FrameRec* __restrict__ fr, QNode* __restrict__ cells, int* __restrict__ d_count,
+__global__ void __launch_bounds__ (TOP_THREADS) k_celltop_down (Params p, const FrameRec* __restrict__ fr, QNode* __restrict__ cells, QNode* __restrict__ cells1,
+                                                               int* __restrict__ d_count,
                                                                QNode* __restrict__ gq, CellTop* __restrict__ tops, int cell_cap,
                                                                int* __restrict__ blist, int bl_stride, unsigned long long* __restrict__ stats,
-                                                               int SL, int qslot, int static_count)
+                                                               int SL, int qslot, int static_count, uint32_t* __restrict__ fold)
 {
   __shared__ __align__ (16) TopSmem S;
   __shared__ Frame s_f_;
@@ -477,8 +519,10 @@ __global__ void __launch_bounds__ (TOP_THREADS) k_celltop_down (Params p, const 
     if (tid < 24) s_pl_[tid >> 2][tid & 3] = fr->pl[tid >> 2][tid & 3];
   }
   int* const cnt_ = d_count + 16 * fr->cset;
+  if (fr->cset) cells = cells1;
   __syncthreads ();
   pdl_wait ();                                          // everything below reads what the previous kernel wrote
+  if (fold && blockIdx.x == 0 && tid == 0) st_release (fold_state (fold, p.C).opened, fr->seq);   // this frame's k_front is complete
   const Frame& f = s_f_;
   unsigned long long upd = 0, vis = 0;
   int count = qslot >= 0 ? cnt_[qslot] : static_count;
@@ -489,7 +533,7 @@ __global__ void __launch_bounds__ (TOP_THREADS) k_celltop_down (Params p, const 
   const double thr[4] = { near_threshold (sizeC), near_threshold (sizeC * 0.5f), near_threshold (sizeC * 0.25f), near_threshold (sizeC * 0.125f) };
   const float thrf[4] = { float_at_least (thr[0]), float_at_least (thr[1]), float_at_least (thr[2]), float_at_least (thr[3]) };
   const bool have_bgra = COLOR && p.color && f.rgba_off >= 0;
-  FrameHot F; F.pix = p.pix;
+  FrameHot F; F.pix = frame_plane (p, fr->cset);
   for (int ci = blockIdx.x; ci < count; ci += gridDim.x)
   {
     __syncthreads ();
@@ -662,9 +706,11 @@ __device__ __forceinline__ int top_fallthrough_new (const Params& p, const Frame
 }
 
 template <bool COLOR>
-__global__ void __launch_bounds__ (128) k_celltop_up (Params gp, const FrameRec* __restrict__ fr, QNode* __restrict__ cells, const int* __restrict__ d_count,
+__global__ void __launch_bounds__ (128) k_celltop_up (Params gp, const FrameRec* __restrict__ fr, QNode* __restrict__ cells, QNode* __restrict__ cells1,
+                                                      const int* __restrict__ d_count,
                                                       const QNode* __restrict__ gq, const CellTop* __restrict__ tops, int cell_cap,
-                                                      unsigned long long* __restrict__ stats, int SL, int qslot, int static_count)
+                                                      unsigned long long* __restrict__ stats, int SL, int qslot, int static_count,
+                                                      uint32_t* __restrict__ fold)
 {
   // Params / Frame live in shared memory here: the out-of-line slow path takes them by reference, which
   // would otherwise make every thread copy the kernel parameters to its stack in the prologue
@@ -688,6 +734,14 @@ __global__ void __launch_bounds__ (128) k_celltop_up (Params gp, const FrameRec*
   unsigned long long upd = 0, vis = 0;
   int count = qslot >= 0 ? d_count[16 * fr->cset + qslot] : static_count;
   if (count > cell_cap) count = cell_cap;
+  if (fr->cset) cells = cells1;
+  uint32_t* const folded = fold ? fold_state (fold, p.C).folded : nullptr;
+  const uint32_t seq = fr->seq;
+  // the cell is final: publish it to the next frame's k_front (the warp's writes to it, then the mark; see FoldState)
+  auto publish = [&] (const QNode& cell) {
+    __syncwarp ();
+    if (folded && lane == 0) { __threadfence (); st_release (&folded[(cell.x << (2 * p.C)) | (cell.y << p.C) | cell.z], seq); }
+  };
   if (fr->timing && blockIdx.x == 0 && threadIdx.x == 0 && fr->kt[1] > fr->kt[0])
   { atomicAdd (&stats[5], fr->kt[1] - fr->kt[0]); atomicAdd (&stats[6], 1ull); }          // device-timed brick kernel of this frame
   const float sizeC = level_size (p, SL);
@@ -701,8 +755,8 @@ __global__ void __launch_bounds__ (128) k_celltop_up (Params gp, const FrameRec*
     int dbg_slow2 = 0, dbg_slow1 = 0, dbg_ft = 0;
     const CellTop* top = tops + ci;
     const int t1 = top->t1slot;
-    if (t1 < 0) continue;                                            // the cell was a leaf: nothing to fold
     const QNode cell = cells[ci];
+    if (t1 < 0) { publish (cell); continue; }                        // the cell was a leaf: nothing to fold
     const float c0[3] = { center1d (p, SL, cell.x), center1d (p, SL, cell.y), center1d (p, SL, cell.z) };
     float2* gdw = p.nodes + (size_t) t1 * BRICK_NODES;
     uchar4* grgb = COLOR ? p.rgb + (size_t) t1 * BRICK_NODES : nullptr;
@@ -802,6 +856,7 @@ __global__ void __launch_bounds__ (128) k_celltop_up (Params gp, const FrameRec*
       else { __threadfence_block (); rc_cell = leaf_visit_warp_bfs (p, f, nc, s_rec[threadIdx.x >> 5], &s_cnt[threadIdx.x >> 5], upd, vis); }
     }
     if (lane == 0 && cell_lvl <= 0) cells[ci].rc = rc_cell;              // (read by k_upper_up when coarse levels lie above the supercell)
+    publish (cell);
     if (p.dbg && lane == 0)
     {
       const long long cD = clock64 ();

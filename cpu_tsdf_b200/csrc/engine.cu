@@ -146,8 +146,23 @@ __global__ void k_cull (Params p, Planes P, unsigned char* __restrict__ mask)
   __syncthreads ();                                                             \
   const Frame& f = s_fr_.f;
 
-__global__ void k_front (Params p, const FrameRec* __restrict__ fr, int cull_blocks, int* __restrict__ list, int* __restrict__ d_count, QNode* __restrict__ q0,
-                         unsigned long long* __restrict__ stats)
+// q0 / q1: the cell queue of a frame with counter set 0 / 1 (null: no queue); fold: the fold marks (FoldState) when the route
+// publishes them, else null.
+//
+// A gated frame (FrameRec::gated, set by the host only when the previous frame's route published the marks) does not wait for
+// the previous frame's k_celltop_up as a whole.  Every block waits for `opened == seq - 1`: the previous frame's k_front is then
+// complete, so its visited marks are final and, through its block 0's griddepcontrol.wait, every frame before it is complete.
+// That is what makes the two counter sets, planes and cell queues enough: what this frame writes was last used by frame
+// seq - 2.  A pixel thread then waits only until the previous frame has folded its own supercell, if that frame visits it: a
+// pre-split reads and writes only its supercell's state (the root split bit, the tier-1 brick, the tier-0 bricks below it) and
+// the brick hash, whose slot order nothing observes.  Only block 0 executes griddepcontrol.wait, last, followed by the
+// frame-begin bookkeeping, so the kernel still completes after the previous frame's last kernel and k_celltop_down's own wait
+// orders all of that frame before this frame's updates; every other block exits as soon as its own work is done.
+// No deadlock: this kernel starts only after every CTA of the previous frame's k_celltop_up has executed
+// griddepcontrol.launch_dependents (its first statement), and so after every CTA of that frame's other kernels has started; all
+// of them are resident, and the frames before it are complete.  A waiting thread therefore waits only on resident work.
+__global__ void k_front (Params p, const FrameRec* __restrict__ fr, int cull_blocks, int* __restrict__ list, int* __restrict__ d_count,
+                         QNode* __restrict__ q0, QNode* __restrict__ q1, uint32_t* __restrict__ fold, unsigned long long* __restrict__ stats)
 {
   pdl_launch_dependents ();
   B2_STAGE_FRAME (fr)
@@ -196,36 +211,80 @@ __global__ void k_front (Params p, const FrameRec* __restrict__ fr, int cull_blo
       }
     }
   }
-  pdl_wait ();                                          // the previous frame's bottom-up sweep has finished
-  int* count = d_count + 16 * s_fr_.cset;
-  int* next_counts = d_count + 16 * (s_fr_.cset ^ 1);
+  const int cset = s_fr_.cset;
+  const bool gated = s_fr_.gated != 0;
+  const FoldState fs = fold_state (fold, p.C);
+  if (gated)
+  {
+    if (threadIdx.x == 0) wait_mark (p, fs.opened, s_fr_.seq - 1u);
+    __syncthreads ();
+  }
+  else pdl_wait ();                                     // the previous frame's bottom-up sweep has finished
+  int* count = d_count + 16 * cset;
+  int* next_counts = d_count + 16 * (cset ^ 1);
   // frame-begin bookkeeping (was a launch of its own): snapshot the cumulative counters, and clear the counter
   // set the NEXT frame will use (the sets alternate, so nothing in this frame touches it)
-  if (blockIdx.x == 0 && threadIdx.x < 16)
-  {
-    if (threadIdx.x < ST_N) stats[ST_N + threadIdx.x] = stats[threadIdx.x];
-    next_counts[threadIdx.x] = 0;
-  }
-  if (!act) return;
+  auto frame_begin = [&] () {
+    if (blockIdx.x == 0 && threadIdx.x < 16)
+    {
+      if (p.dbg && threadIdx.x == 0) atomicAdd (&p.dbg[gated ? 11 : 12], 1ull);   // which k_front ran (b200tsdf_debug_timing)
+      if (threadIdx.x < ST_N) stats[ST_N + threadIdx.x] = stats[threadIdx.x];
+      next_counts[threadIdx.x] = 0;
+    }
+  };
+  if (!gated) frame_begin ();
   if (cull)
   {
-    int k = atomicAdd (count, 1);
-    list[k] = i;
-    if (q0)
+    if (act)
     {
-      NodePos nd;
-      if (!locate_node (p, p.C, x, y, z, nd)) { raise_err (p, ERR_MISSING_BRICK); nd.slot = -1; nd.idx = 0; }
-      QNode e; e.x = x; e.y = y; e.z = z; e.slot = nd.slot; e.idx = nd.idx; e.kind = KIND_DONE; e.child_base = -1; e.rc = 0;
-      q0[k] = e;
+      int k = atomicAdd (count, 1);
+      list[k] = i;
+      if (q0)
+      {
+        NodePos nd;
+        if (!locate_node (p, p.C, x, y, z, nd)) { raise_err (p, ERR_MISSING_BRICK); nd.slot = -1; nd.idx = 0; }
+        QNode e; e.x = x; e.y = y; e.z = z; e.slot = nd.slot; e.idx = nd.idx; e.kind = KIND_DONE; e.child_base = -1; e.rc = 0;
+        (cset ? q1 : q0)[k] = e;
+      }
+      if (fold) fs.visited[(size_t) cset * (n * n * n) + i] = s_fr_.seq;
     }
-    return;
   }
-  // the pixel plane the observations of this frame read (Params::pix): a bit copy of every pixel, NaN depths, points
-  // outside the volume and points in another shard's cells included, because an observation may project onto any pixel.
-  // Written only past pdl_wait: the previous frame's readers are done.
-  if (p.color) reinterpret_cast<uint2*> (p.pix)[i] = make_uint2 (zb, bgra);
-  else p.pix[i] = zb;
-  if (split_it) presplit_point (p, fx_, fy_, fz_);
+  else
+  {
+    // the pixel plane the observations of this frame read (frame_plane): a bit copy of every pixel, NaN depths, points
+    // outside the volume and points in another shard's cells included, because an observation may project onto any pixel.
+    // The previous readers of this plane are frame seq - 2's kernels, which are complete.
+    if (act)
+    {
+      uint32_t* pix = frame_plane (p, cset);
+      if (p.color) reinterpret_cast<uint2*> (pix)[i] = make_uint2 (zb, bgra);
+      else pix[i] = zb;
+    }
+    if (gated)
+    {
+      // wait for the previous frame's fold of this pixel's supercell, one poll per distinct cell of the warp
+      const int sh = p.L - p.C;
+      const int cell = split_it ? (((fx_ >> sh) * n + (fy_ >> sh)) * n + (fz_ >> sh)) : -1;
+      const uint32_t prev = s_fr_.seq - 1u;
+      const uint32_t* prev_visited = fs.visited + (size_t) (cset ^ 1) * (n * n * n);
+      const int lane = threadIdx.x & 31;
+      unsigned todo = __ballot_sync (0xffffffffu, cell >= 0);
+      while (todo)
+      {
+        const int leader = __ffs (todo) - 1;
+        const int c = __shfl_sync (0xffffffffu, cell, leader);
+        todo &= ~__ballot_sync (0xffffffffu, cell == c);
+        if (lane == leader && ld_relaxed (prev_visited + c) == prev) wait_mark (p, fs.folded + c, prev);
+      }
+      __syncwarp ();
+    }
+    if (split_it) presplit_point (p, fx_, fy_, fz_);
+  }
+  if (gated && blockIdx.x == 0 && threadIdx.x < 16)
+  {
+    pdl_wait ();                                        // the previous frame's bottom-up sweep has finished
+    frame_begin ();
+  }
 }
 
 // general path: one thread per culled coarse cell runs updateVoxel depth-first.  The frame and its counter set come from
@@ -709,6 +768,11 @@ struct b200tsdf
   // supercell path: sl = level of the tier-1 roots, nup = coarse levels above them (swept by k_upper_*), super_static = number of
   // supercells when every tier-1 root is one (coarse cells inside the brick)
   int cell_cap = 0; QNode* d_cellq = nullptr; size_t cellq_cap = 0; CellTop* d_celltop = nullptr; QNode* d_superq = nullptr;
+  // the per-supercell gate of k_front (FoldState, brick_kernels.cuh): on the route whose supercells are the culled coarse cells
+  // the fold marks, and the cell queue of frames with counter set 1 (Q.q[0] serves set 0)
+  uint32_t* d_fold = nullptr; size_t fold_cap = 0; QNode* d_q1 = nullptr; size_t q1_cap = 0;
+  uint32_t frame_seq = 0;        // FrameRec::seq of the last frame
+  bool fold_prev = false;        // the last frame's route published fold marks (the next one on that route may be gated)
   bool top_path = false; int sl = 0, nup = 0, super_static = 0;
   bool fast_path = false; int force_general = 0;
   // device copy of Params (the rare out-of-line paths read it through a pointer) and the ring of per-frame records
@@ -830,6 +894,7 @@ int check_device_err (b200tsdf* h)
   if (e & ERR_POOL_FULL) return h->fail (B200TSDF_ENOMEM, "brick pool exhausted (raise pool_log2)");
   if (e & ERR_MISSING_BRICK) return h->fail (B200TSDF_ESTATE, "internal: split node without brick");
   if (e & ERR_QUEUE_FULL) return h->fail (B200TSDF_ENOMEM, "internal: work queue overflow");
+  if (e & ERR_FOLD_WAIT) return h->fail (B200TSDF_ESTATE, "internal: k_front waited too long for the previous frame's fold");
   return 0;
 }
 
@@ -843,6 +908,7 @@ int pending_device_err (b200tsdf* h)
   if (!e) return 0;
   if (e & ERR_POOL_FULL) return h->fail (B200TSDF_ENOMEM, "brick pool exhausted in an earlier frame (raise pool_log2); the volume is incomplete");
   if (e & ERR_MISSING_BRICK) return h->fail (B200TSDF_ESTATE, "internal: split node without brick (earlier frame)");
+  if (e & ERR_FOLD_WAIT) return h->fail (B200TSDF_ESTATE, "internal: k_front waited too long for the previous frame's fold (earlier frame)");
   return h->fail (B200TSDF_ENOMEM, "internal: work queue overflow in an earlier frame; the volume is incomplete");
 }
 void note_device_err (b200tsdf* h, cudaStream_t s) { cudaMemcpyAsync (h->h_err, h->d_err, sizeof (int), cudaMemcpyDeviceToHost, s); }
@@ -1029,6 +1095,7 @@ void b200tsdf_destroy (b200tsdf_t* h)
   for (int i = 0; i < BATCH_SEGS; ++i) if (h->ev_bring[i]) cudaEventDestroy (h->ev_bring[i]);
   for (int i = 0; i < 2; ++i) if (h->ev_half_done[i]) cudaEventDestroy (h->ev_half_done[i]);
   cudaFree (h->d_frame[0]); cudaFree (h->d_frame[1]); cudaFree (h->q_mem); cudaFree (h->d_blist); cudaFree (h->d_cellq); cudaFree (h->d_superq); cudaFree (h->d_celltop);
+  cudaFree (h->d_fold); cudaFree (h->d_q1);
   for (int i = 0; i < 2; ++i) { if (h->ev_copied[i]) cudaEventDestroy (h->ev_copied[i]); if (h->ev_consumed[i]) cudaEventDestroy (h->ev_consumed[i]); }
   if (h->ev_t0) cudaEventDestroy (h->ev_t0); if (h->ev_t1) cudaEventDestroy (h->ev_t1);
   if (h->ev_p0) cudaEventDestroy (h->ev_p0); if (h->ev_p1) cudaEventDestroy (h->ev_p1);
@@ -1103,7 +1170,7 @@ int b200tsdf_reset (b200tsdf_t* h)
     CK (cudaMalloc (&h->d_culled, ncells * sizeof (int)));
     h->culled_cap = ncells;
   }
-  const size_t pix_bytes = (size_t) np.width * np.height * (color ? 8 : 4);
+  const size_t pix_bytes = 2 * (size_t) np.width * np.height * (color ? 8 : 4);   // two planes alternate by counter set (frame_plane)
   if (pix_bytes > h->pix_cap)
   {
     h->has_volume = false;                                 // the frames' launches need the plane
@@ -1162,6 +1229,23 @@ int b200tsdf_reset (b200tsdf_t* h)
       }
       if (h->super_static && !h->d_superq) CK (cudaMalloc (&h->d_superq, 4096 * sizeof (QNode)));
     }
+    if (h->top_path && h->sl == np.C)
+    {
+      // the per-supercell gate of k_front (FoldState): fold marks over the coarse cells, and a second level-C queue
+      const size_t fw = fold_words (np.C);
+      if (fw > h->fold_cap)
+      {
+        cudaFree (h->d_fold); h->d_fold = nullptr; h->fold_cap = 0;
+        CK (cudaMalloc (&h->d_fold, fw * sizeof (uint32_t)));
+        h->fold_cap = fw;
+      }
+      if ((size_t) h->Q.cap[0] > h->q1_cap)
+      {
+        cudaFree (h->d_q1); h->d_q1 = nullptr; h->q1_cap = 0;
+        CK (cudaMalloc (&h->d_q1, (size_t) h->Q.cap[0] * sizeof (QNode)));
+        h->q1_cap = h->Q.cap[0];
+      }
+    }
     size_t bl = h->q_levels ? caps[h->q_levels - 1] : 0;
     if (h->top_path) bl = std::max (bl, (size_t) h->cell_cap * 512);
     if (bl > h->blist_cap)
@@ -1203,6 +1287,8 @@ int b200tsdf_reset (b200tsdf_t* h)
   *h->h_err = 0;
   CK (cudaMemsetAsync (h->d_count, 0, 64 * sizeof (int), s));
   h->count_set = 0;
+  if (h->d_fold) CK (cudaMemsetAsync (h->d_fold, 0, h->fold_cap * sizeof (uint32_t), s));
+  h->fold_prev = false;
   CK (cudaMemsetAsync (h->d_stats, 0, ST_TOTAL * sizeof (unsigned long long), s));
   h->kring_pending = 0; h->kring_head = 0;
   if (Rtop < C) k_insert_top_bricks<<<(unsigned) ((root_n + 127) / 128), 128, 0, s>>> (p);
@@ -1217,6 +1303,12 @@ int b200tsdf_reset (b200tsdf_t* h)
 }
 
 // ---- integrateCloud (hpp:48-103) ------------------------------------------------------------------
+// The route whose kernels publish the fold marks of FoldState (brick_kernels.cuh), and whose k_front may therefore wait per
+// supercell: the supercells are the culled coarse cells (C == SL, no k_upper_* levels) and the frame's last kernel is
+// k_celltop_up.  Other routes wait for the previous frame's last kernel before any octree work.  It follows the handle's
+// current route, including the switch to the general kernel after out-of-domain writes.
+static bool publishes_folds (const b200tsdf* h) { return h->fast_path && h->top_path && h->sl == h->p.C; }
+
 // The frame's parameters (pose, planes, cloud pointer, counter set) are written into a FrameRec; the hot kernels
 // read it from the device ring, so the very same launches can be captured once into a CUDA graph and replayed.
 static void fill_rec (b200tsdf* h, FrameRec& r, const unsigned char* d_pts, size_t stride, int xyz_off, int rgba_off, int W, int H, const double* pose)
@@ -1227,7 +1319,11 @@ static void fill_rec (b200tsdf* h, FrameRec& r, const unsigned char* d_pts, size
   h->count_set ^= 1;                                                  // counter sets alternate between frames
   r.cset = h->count_set;
   r.timing = h->time_frames ? 1 : 0;
-  r.pad_[0] = r.pad_[1] = 0; r.kt[0] = r.kt[1] = 0;
+  r.seq = ++h->frame_seq;
+  const bool pub = publishes_folds (h);
+  r.gated = pub && h->fold_prev;                                      // (the previous frame's kernels publish the marks it waits on)
+  h->fold_prev = pub;
+  r.kt[0] = r.kt[1] = 0;
 }
 
 // the launches of one frame; every kernel reads the frame from *d_rec, so the launches can be captured and replayed.
@@ -1240,11 +1336,16 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, boo
   const Params& p = h->p;
   const int npix = h->cfg.image_width * h->cfg.image_height;   // (every frame has this size: check_cloud_layout)
   const int ncells = 1 << (3 * p.C);
+  // on the route that publishes fold marks, frames alternate between two cell queues (k_front fills the next frame's while
+  // this frame's k_celltop_up still reads its own); other routes use Q.q[0] for both counter sets
+  const bool pub = publishes_folds (h);
+  uint32_t* const fold = pub ? h->d_fold : nullptr;
+  QNode* const q1 = pub ? h->d_q1 : h->Q.q[0];
   {
     const int cull_blocks = (ncells + 255) / 256;
     const dim3 grid (cull_blocks + (npix + 255) / 256);
-    if (front_pdl) CK (launch_pdl (k_front, grid, dim3 (256), s, p, d_rec, cull_blocks, h->d_culled, h->d_count, h->Q.q[0], h->d_stats));
-    else k_front<<<grid, 256, 0, s>>> (p, d_rec, cull_blocks, h->d_culled, h->d_count, h->Q.q[0], h->d_stats);
+    if (front_pdl) CK (launch_pdl (k_front, grid, dim3 (256), s, p, d_rec, cull_blocks, h->d_culled, h->d_count, h->Q.q[0], q1, fold, h->d_stats));
+    else k_front<<<grid, 256, 0, s>>> (p, d_rec, cull_blocks, h->d_culled, h->d_count, h->Q.q[0], q1, fold, h->d_stats);
   }
   h->launches += 1;
   int kr = -1;
@@ -1264,7 +1365,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, boo
       QNode* cells = h->super_static ? h->d_superq : h->Q.q[h->nup];
       const int qslot = h->super_static ? -1 : h->nup;
       auto kd = p.color ? k_celltop_down<true> : k_celltop_down<false>;
-      CK (launch_pdl (kd, dim3 (h->sm_count * 4), dim3 (TOP_THREADS), s, p, d_rec, cells, h->d_count, h->d_cellq, h->d_celltop, h->cell_cap, h->d_blist, (int) h->blist_cap, h->d_stats, h->sl, qslot, h->super_static));
+      CK (launch_pdl (kd, dim3 (h->sm_count * 4), dim3 (TOP_THREADS), s, p, d_rec, cells, pub ? q1 : cells, h->d_count, h->d_cellq, h->d_celltop, h->cell_cap, h->d_blist, (int) h->blist_cap, h->d_stats, h->sl, qslot, h->super_static, fold));
       h->launches++;
       bq = h->d_cellq;
     }
@@ -1288,7 +1389,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, boo
       QNode* cells = h->super_static ? h->d_superq : h->Q.q[h->nup];
       const int qslot = h->super_static ? -1 : h->nup;
       auto ku = p.color ? k_celltop_up<true> : k_celltop_up<false>;
-      CK (launch_pdl (ku, dim3 (h->sm_count), dim3 (128), s, p, d_rec, cells, (const int*) h->d_count, (const QNode*) h->d_cellq, (const CellTop*) h->d_celltop, h->cell_cap, h->d_stats, h->sl, qslot, h->super_static));
+      CK (launch_pdl (ku, dim3 (h->sm_count), dim3 (128), s, p, d_rec, cells, pub ? q1 : cells, (const int*) h->d_count, (const QNode*) h->d_cellq, (const CellTop*) h->d_celltop, h->cell_cap, h->d_stats, h->sl, qslot, h->super_static, fold));
       h->launches++;
       for (int li = h->nup - 1; li >= 0; --li) { k_upper_up<<<h->sm_count * 2, 128, 0, s>>> (p, d_rec, h->Q, li, h->d_stats); h->launches++; }
     }
@@ -2368,7 +2469,8 @@ extern "C" {
 
 // Diagnostics (not part of include/b200tsdf.h): phase timing of k_celltop_up.  First call arms it; every call returns and
 // clears the 16 counters ([0..5] max SM cycles << 32 | tag of total / level-3 / level-2 / level-1 / cell / wait-before-first-cell,
-// [6..10] slow level-2 nodes, slow level-1 nodes, cell leaf visits, cell fall-throughs, cells folded).
+// [6..10] slow level-2 nodes, slow level-1 nodes, cell leaf visits, cell fall-throughs, cells folded; [11] frames whose k_front
+// waited per supercell, [12] frames whose k_front waited for the previous frame's last kernel).
 int b200tsdf_debug_timing (b200tsdf_t* h, unsigned long long* out16)
 {
   if (!h || !out16) return B200TSDF_EINVAL;

@@ -51,7 +51,7 @@ constexpr int BRICK_SPLIT_WORDS = 20;   // word 0: 8 bits, words 1-2: 64 bits, w
 constexpr uint64_t KEY_EMPTY = 0ull;
 constexpr int MAX_PROBE = 4096;
 
-enum ErrBits { ERR_POOL_FULL = 1, ERR_MISSING_BRICK = 2, ERR_QUEUE_FULL = 4 };
+enum ErrBits { ERR_POOL_FULL = 1, ERR_MISSING_BRICK = 2, ERR_QUEUE_FULL = 4, ERR_FOLD_WAIT = 8 };
 
 // ---- rounding-exact scalar ops ------------------------------------------------------------
 B2_HD float fadd (float a, float b)
@@ -164,7 +164,7 @@ struct Params
   unsigned char* work;        // [pool] finest-tier bricks: interior level-2 nodes seen by the last update (scheduling hint only)
   int* err;                   // device error bits
   unsigned long long* dbg;    // optional phase timing of k_celltop_up (b200tsdf_debug_timing), normally null
-  uint32_t* pix;              // [width * height] pixel plane of the current frame, written by k_front: {z bits, bgra} per pixel
+  uint32_t* pix;              // [2][width * height] pixel planes (frame_plane), written by k_front: {z bits, bgra} per pixel
                               // with colour, z bits alone without (read by the fast observation, obs_fast.cuh)
 };
 
