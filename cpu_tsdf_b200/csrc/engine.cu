@@ -38,32 +38,41 @@ namespace {
 
 struct Planes { float pl[6][4]; };
 
-// A device buffer owned by one host call: freed when it goes out of scope, so error returns free it too.  Work queued on
-// its stream may still read it, so the stream is drained before the memory is released.
+// A device buffer, freed when it goes out of scope, so error returns free it too.  One owned by a host call names its
+// stream: work queued there may still read the buffer, so the stream is drained before the memory is released.  One of the
+// handle has no stream: it is released by grow, or after b200tsdf_destroy has synchronised the handle's streams.
 template <typename T>
 struct DevBuf
 {
   T* p = nullptr;
-  cudaStream_t s;
+  size_t cap = 0;                               // elements allocated
+  cudaStream_t s = nullptr;
+  DevBuf () = default;
   explicit DevBuf (cudaStream_t stream) : s (stream) {}
-  DevBuf (DevBuf&& o) noexcept : p (o.p), s (o.s) { o.p = nullptr; }
-  DevBuf& operator= (DevBuf&& o) noexcept { std::swap (p, o.p); std::swap (s, o.s); return *this; }
+  DevBuf (DevBuf&& o) noexcept : p (o.p), cap (o.cap), s (o.s) { o.p = nullptr; o.cap = 0; }
+  DevBuf& operator= (DevBuf&& o) noexcept { std::swap (p, o.p); std::swap (cap, o.cap); std::swap (s, o.s); return *this; }
   DevBuf (const DevBuf&) = delete;
   DevBuf& operator= (const DevBuf&) = delete;
   ~DevBuf () { release (); }
   void release ()
   {
     if (!p) return;
-    cudaStreamSynchronize (s);
+    if (s) cudaStreamSynchronize (s);
     cudaFree (p);
-    p = nullptr;
+    p = nullptr; cap = 0;
   }
-  cudaError_t alloc (size_t n)                  // n elements; n == 0 leaves the buffer null
+  cudaError_t alloc (size_t n)                  // exactly n elements; n == 0 leaves the buffer null
   {
     release ();
-    if (!n) return cudaSuccess;
+    return grow (n);
+  }
+  cudaError_t grow (size_t n)                   // at least n elements: kept when they fit, else freed before the new allocation
+  {
+    if (n <= cap) return cudaSuccess;
+    release ();
     const cudaError_t e = cudaMalloc (&p, n * sizeof (T));
-    if (e != cudaSuccess) p = nullptr;
+    if (e != cudaSuccess) { p = nullptr; return e; }
+    cap = n;
     return e;
   }
   cudaError_t upload (const std::vector<T>& v)  // a device copy of v
@@ -74,6 +83,33 @@ struct DevBuf
   }
   operator T* () const { return p; }
 };
+
+// Pinned host memory of the handle, freed with it
+template <typename T>
+struct Pinned
+{
+  T* p = nullptr;
+  Pinned () = default;
+  Pinned (const Pinned&) = delete;
+  Pinned& operator= (const Pinned&) = delete;
+  ~Pinned () { if (p) cudaFreeHost (p); }
+  cudaError_t alloc (size_t n) { return cudaHostAlloc ((void**) &p, n * sizeof (T), cudaHostAllocDefault); }
+  operator T* () const { return p; }
+};
+
+// A stream or event of the handle, destroyed with it
+template <typename X, cudaError_t (*destroy) (X)>
+struct Owned
+{
+  X x = nullptr;
+  Owned () = default;
+  Owned (const Owned&) = delete;
+  Owned& operator= (const Owned&) = delete;
+  ~Owned () { if (x) destroy (x); }
+  operator X () const { return x; }
+};
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
 
 // d_stats[0..ST_N) are cumulative since reset(); [ST_N..2*ST_N) is the snapshot taken at the start of
 // the current frame (so last-frame = cum - prev without a host round trip); the last slot is scratch
@@ -703,6 +739,10 @@ __global__ void k_leaves_level (Params gp, int level, unsigned long long count, 
 struct Staging
 {
   unsigned char* p = nullptr; size_t bytes = 0;
+  Staging () = default;
+  Staging (const Staging&) = delete;
+  Staging& operator= (const Staging&) = delete;
+  ~Staging () { release (); }
   int alloc (size_t n)
   {
     release ();
@@ -738,79 +778,91 @@ struct Staging
   }
 };
 
+// The volume's device storage (the storage pointers of Params, see b200tsdf::storage_into) for one pool size, root-array size
+// and payload; assigning a fresh Volume frees it
+struct Volume
+{
+  size_t pool = 0, root_n = 0;
+  bool color = false, var = false, norm = false;
+  DevBuf<uint64_t> keys; DevBuf<float2> nodes; DevBuf<uint32_t> split; DevBuf<unsigned char> work;
+  DevBuf<uchar4> rgb; DevBuf<float> M; DevBuf<int> ns; DevBuf<float4> rgbn;
+  DevBuf<float2> root_dw; DevBuf<uint32_t> root_split; DevBuf<uchar4> root_rgb; DevBuf<float4> root_rgbn;
+  DevBuf<float> root_M; DevBuf<int> root_ns;
+};
+
+constexpr int CELL_CAP = 16384;  // supercells of one frame on the supercell path (d_celltop; d_cellq holds 585 entries each)
+
 struct b200tsdf
 {
+  // declared first, so that they are destroyed last: b200tsdf_destroy synchronises them and then frees everything below
+  Stream stream, copy_stream, gather_stream;   // compute | H2D uploads | pack + NVLink all-gather
   b200tsdf_config cfg_pending{}, cfg{};
   bool has_volume = false;
   Params p{};
   int device = 0, sm_count = 0;            // cudaDevAttrMultiProcessorCount, read in b200tsdf_create
-  cudaStream_t stream = nullptr, copy_stream = nullptr, gather_stream = nullptr;   // compute | H2D uploads | pack + NVLink all-gather
-  size_t pool = 0;
-  bool alloc_color = false, alloc_var = false, alloc_norm = false;
-  size_t root_n = 0;
-  int* d_err = nullptr;
-  unsigned char* d_frame[2] = { nullptr, nullptr };
-  size_t frame_cap = 0;
-  cudaEvent_t ev_copied[2] = { nullptr, nullptr }, ev_consumed[2] = { nullptr, nullptr };
-  cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
+  Volume vol;
+  DevBuf<int> d_err;
+  DevBuf<unsigned char> d_frame[2];
+  Event ev_copied[2], ev_consumed[2];
+  Event ev_t0, ev_t1;
   uint64_t frame_no = 0;
   int count_set = 0;             // which of the two per-frame counter sets the last frame used
-  int* d_culled = nullptr; int* d_count = nullptr; unsigned long long* d_stats = nullptr;
-  size_t culled_cap = 0;
-  uint32_t* d_pix = nullptr; size_t pix_cap = 0;   // Params::pix (bytes allocated, grow-only)
+  DevBuf<int> d_culled; DevBuf<int> d_count; DevBuf<unsigned long long> d_stats;
+  DevBuf<uint32_t> d_pix;        // Params::pix (grow-only)
   bool timed = false;
   bool time_frames = false;      // set between profile_begin / profile_end: per-frame event records (ev_t0/ev_t1 and the ring around the dominant kernel)
   bool is_empty = true;          // TSDFVolumeOctree::is_empty_ (cpp:205, hpp:101)
-  // fast-path work queues (levels C .. L-3)
-  Queues Q{}; int q_levels = 0; QNode* q_mem = nullptr; size_t q_mem_cap = 0;
-  int* d_blist = nullptr; size_t blist_cap = 0;
+  // fast-path work queues (levels C .. L-3), and the lists of block roots, BL_CLASSES lists of blist_cap () entries
+  Queues Q{}; int q_levels = 0; DevBuf<QNode> q_mem;
+  DevBuf<int> d_blist;
+  int blist_cap () const { return (int) (d_blist.cap / BL_CLASSES); }
   // fused per-cell upper sweeps (coarse cells are the top-tier roots and the block roots are <= 3 levels below)
   // supercell path: sl = level of the tier-1 roots, nup = coarse levels above them (swept by k_upper_*), super_static = number of
   // supercells when every tier-1 root is one (coarse cells inside the brick)
-  int cell_cap = 0; QNode* d_cellq = nullptr; size_t cellq_cap = 0; CellTop* d_celltop = nullptr; QNode* d_superq = nullptr;
+  DevBuf<QNode> d_cellq; DevBuf<CellTop> d_celltop; DevBuf<QNode> d_superq;
   // the per-supercell gate of k_front (FoldState, brick_kernels.cuh): on the route whose supercells are the culled coarse cells
   // the fold marks, and the cell queue of frames with counter set 1 (Q.q[0] serves set 0)
-  uint32_t* d_fold = nullptr; size_t fold_cap = 0; QNode* d_q1 = nullptr; size_t q1_cap = 0;
+  DevBuf<uint32_t> d_fold; DevBuf<QNode> d_q1;
   uint32_t frame_seq = 0;        // FrameRec::seq of the last frame
   bool fold_prev = false;        // the last frame's route published fold marks (the next one on that route may be gated)
   bool top_path = false; int sl = 0, nup = 0, super_static = 0;
-  bool fast_path = false; int force_general = 0;
+  bool fast_path = false;
   // device copy of Params (the rare out-of-line paths read it through a pointer) and the ring of per-frame records
-  Params* d_params = nullptr;
-  unsigned long long* d_dbg = nullptr;     // phase-timing counters of k_celltop_up once b200tsdf_debug_timing armed them
-  int* h_err = nullptr;                    // pinned image of the device error bits, refreshed behind every frame (see note_device_err)
-  FrameRec* d_ring = nullptr; FrameRec* h_ring = nullptr; uint64_t ring_seq = 0;
-  cudaEvent_t ev_ring[2] = { nullptr, nullptr };
+  DevBuf<Params> d_params;
+  DevBuf<unsigned long long> d_dbg;        // phase-timing counters of k_celltop_up once b200tsdf_debug_timing armed them
+  Pinned<int> h_err;                       // pinned image of the device error bits, refreshed behind every frame (see note_device_err)
+  DevBuf<FrameRec> d_ring; Pinned<FrameRec> h_ring; uint64_t ring_seq = 0;
+  Event ev_ring[2];
   // batches (b200tsdf_integrate_batch_device): their own record ring, used half by half, and one captured graph per
   // (half, batch size); a graph is valid until the next reset()
   // device slots: two halves of FRAME_RING / 2 records, reused in stream order; host staging: BATCH_SEGS segments written round
   // robin — the host only waits when it is BATCH_SEGS batches ahead of the device
   // (each half and each segment is BRING_SPAN slots: the frame records, then the organise block of an unorganised batch)
-  FrameRec* d_bring = nullptr; FrameRec* h_bring = nullptr; int bring_half = 0; int bring_seg = 0; bool bring_used[BATCH_SEGS] = {};
-  cudaEvent_t ev_bring[BATCH_SEGS] = {};
-  cudaEvent_t ev_half_done[2] = { nullptr, nullptr }; bool half_used[2] = { false, false };
+  DevBuf<FrameRec> d_bring; Pinned<FrameRec> h_bring; int bring_half = 0; int bring_seg = 0; bool bring_used[BATCH_SEGS] = {};
+  Event ev_bring[BATCH_SEGS];
+  Event ev_half_done[2]; bool half_used[2] = { false, false };
   cudaGraphExec_t batch_exec[2][FRAME_RING / 2 + 1] = {};
   cudaGraphExec_t unorg_exec[2][FRAME_RING / 2 + 1] = {};   // the same with the three organise launches in front
   // unorganised batches: the keys, filled counters and 16-byte organised images of one record half (organise and fuse of both
-  // halves run on `stream`, so one set serves both); allocated at the first unorganised integrate, freed by reset() and destroy
-  unsigned char* d_org = nullptr;
+  // halves run on `stream`, so one set serves both); allocated at the first unorganised integrate, freed by reset()
+  DevBuf<unsigned char> d_org;
   // multi-GPU (multigpu.cuh): NCCL communicator (opaque here), row-sliced uploads
   void* comm = nullptr; int comm_rank = 0, comm_size = 1;
-  unsigned char* d_rows_raw[2] = { nullptr, nullptr }; unsigned char* d_rows_full[2] = { nullptr, nullptr };
-  size_t rows_raw_cap = 0, rows_full_cap = 0; int rows_set = 0; bool rows_used[2] = { false, false }; int rows_last_up[2] = { 0, 0 };
+  DevBuf<unsigned char> d_rows_raw[2], d_rows_full[2];
+  int rows_set = 0; bool rows_used[2] = { false, false }; int rows_last_up[2] = { 0, 0 };
   int rows_chunk = 0;            // frames per upload/fuse pipeline stage of b200tsdf_integrate_batch_rows (B200TSDF_ROWS_CHUNK=1..32; 0: 1 or 2 with host packing, else 8)
-  cudaEvent_t ev_rows_up[2][32] = {}, ev_rows_ready[2][32] = {}, ev_rows_done[2] = { nullptr, nullptr };
+  Event ev_rows_up[2][32], ev_rows_ready[2][32], ev_rows_done[2];
   // host packing of the uploaded rows (host_pack.h): pinned staging per buffer set, the pool is created on first use
   int host_pack = -1;            // B200TSDF_HOST_PACK: 1 pack on the host, 0 upload the caller's points as they are (packed on the device when gathered); -1 by rank count
   int pack_threads = 0;          // B200TSDF_PACK_THREADS (0 = min (16, hardware threads / (2 ranks)))
   b2host::PackPool* pack_pool = nullptr;
-  Staging h_pack[2]; size_t pack_cap = 0;
-  Staging h_fpack[2];            // the same for the frame-at-a-time upload (d_frame[]), frame_cap bytes each
+  Staging h_pack[2];
+  Staging h_fpack[2];            // the same for the frame-at-a-time upload (d_frame[]), as many bytes as each of d_frame[] holds
   long long nvlink_bytes = 0, prof_nvlink0 = 0;
   int launches_per_frame = 0; long long graph_launches = 0, prof_graph0 = 0;
   // measurement
-  cudaEvent_t ev_p0 = nullptr, ev_p1 = nullptr;
-  cudaEvent_t kring[KRING][2] = {};
+  Event ev_p0, ev_p1;
+  Event kring[KRING][2];
   int kring_head = 0, kring_pending = 0;
   double prof_ms_kernel = 0; long long prof_kernel_launches = 0, prof_frames = 0;
   long long launches = 0, prof_launch0 = 0, h2d_bytes = 0, d2h_bytes = 0, prof_h2d0 = 0, prof_d2h0 = 0;
@@ -830,40 +882,36 @@ struct b200tsdf
   void* mesh_v = nullptr; void* mesh_c = nullptr;           // b200tsdf_mesh results (malloc'ed)
   void* leaf_xyz = nullptr; void* leaf_ijk = nullptr;       // b200tsdf_voxel_centers / _occupied_voxel_indices results
   // grow-only device scratch for the read-side calls (queries, render): no allocation per call
-  unsigned char* d_scratch = nullptr; size_t scratch_cap = 0;
-  // render records (b200tsdf_render_batch_device), allocated at the first render: one device chunk, reused in stream order,
-  // and RENDER_SEGS pinned staging segments written round robin, each free again once the copy that read it has run
-  RenderParams* d_rrec = nullptr; RenderParams* h_rrec = nullptr; int rrec_seg = 0; bool rrec_used[RENDER_SEGS] = {};
-  cudaEvent_t ev_rrec[RENDER_SEGS] = {};
+  DevBuf<unsigned char> d_scratch;
+  // render records (b200tsdf_render_batch_device): one device chunk, reused in stream order, and RENDER_SEGS pinned staging
+  // segments written round robin, each free again once the copy that read it has run
+  DevBuf<RenderParams> d_rrec; Pinned<RenderParams> h_rrec; int rrec_seg = 0; bool rrec_used[RENDER_SEGS] = {};
+  Event ev_rrec[RENDER_SEGS];
   int scratch (size_t bytes)
   {
-    if (bytes <= scratch_cap) return 0;
-    cudaFree (d_scratch); d_scratch = nullptr; scratch_cap = 0;
-    size_t want = bytes + bytes / 2 + 4096;
-    if (cudaMalloc (&d_scratch, want) != cudaSuccess) return fail (B200TSDF_ENOMEM, "device scratch allocation failed");
-    scratch_cap = want;
+    if (bytes <= d_scratch.cap) return 0;
+    if (d_scratch.grow (bytes + bytes / 2 + 4096)) return fail (B200TSDF_ENOMEM, "device scratch allocation failed");
     return 0;
   }
+  // the device pointers of Params: the volume storage and the handle's buffers the kernels write
+  void storage_into (Params& q) const
+  {
+    q.keys = vol.keys; q.nodes = vol.nodes; q.split = vol.split; q.work = vol.work;
+    q.rgb = vol.rgb; q.M = vol.M; q.ns = vol.ns; q.rgbn = vol.rgbn;
+    q.root_dw = vol.root_dw; q.root_split = vol.root_split; q.root_rgb = vol.root_rgb; q.root_rgbn = vol.root_rgbn;
+    q.root_M = vol.root_M; q.root_ns = vol.root_ns;
+    q.err = d_err; q.pix = d_pix; q.dbg = d_dbg;
+  }
+  ~b200tsdf ();
 
   int fail (int code, const std::string& m) { err = m; return code; }
 };
 
 namespace {
 
-void free_volume (b200tsdf* h)
-{
-  cudaFree (h->p.work); h->p.work = nullptr;
-  cudaFree (h->p.keys); cudaFree (h->p.nodes); cudaFree (h->p.split); cudaFree (h->p.rgb); cudaFree (h->p.M); cudaFree (h->p.ns);
-  cudaFree (h->p.root_dw); cudaFree (h->p.root_split); cudaFree (h->p.root_rgb); cudaFree (h->p.root_M); cudaFree (h->p.root_ns);
-  cudaFree (h->p.rgbn); cudaFree (h->p.root_rgbn); h->p.rgbn = nullptr; h->p.root_rgbn = nullptr;
-  h->p.keys = nullptr; h->p.nodes = nullptr; h->p.split = nullptr; h->p.rgb = nullptr; h->p.M = nullptr; h->p.ns = nullptr;
-  h->p.root_dw = nullptr; h->p.root_split = nullptr; h->p.root_rgb = nullptr; h->p.root_M = nullptr; h->p.root_ns = nullptr;
-  h->pool = 0; h->root_n = 0;
-}
-
 // launch with programmatic stream serialization (see pdl_wait in brick_kernels.cuh); also valid inside a stream capture
 template <typename... KArgs, typename... Args>
-cudaError_t launch_pdl (void (*kernel) (KArgs...), dim3 grid, dim3 block, cudaStream_t s, Args... args)
+cudaError_t launch_pdl (void (*kernel) (KArgs...), dim3 grid, dim3 block, cudaStream_t s, const Args&... args)
 {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = 0; cfg.stream = s;
@@ -925,12 +973,12 @@ void fill_frame (const b200tsdf* h, Frame& f, const unsigned char* d_pts, size_t
 // The list lives until the next use of the scratch.
 int list_bricks (b200tsdf* h, int*& list)
 {
-  if (int rc = h->scratch (h->pool * sizeof (int))) return rc;
-  list = (int*) h->d_scratch;
+  if (int rc = h->scratch (h->vol.pool * sizeof (int))) return rc;
+  list = (int*) h->d_scratch.p;
   int* d_n = h->d_count + 40;
   cudaStream_t s = h->stream;
   CK (cudaMemsetAsync (d_n, 0, sizeof (int), s));
-  k_list_bricks<<<(unsigned) ((h->pool + 255) / 256), 256, 0, s>>> (h->p, list, d_n);
+  k_list_bricks<<<(unsigned) ((h->vol.pool + 255) / 256), 256, 0, s>>> (h->p, list, d_n);
   int nb = 0;
   CK (cudaMemcpyAsync (&nb, d_n, sizeof (int), cudaMemcpyDeviceToHost, s));
   CK (cudaStreamSynchronize (s));
@@ -1009,7 +1057,21 @@ int sorted_records_host (b200tsdf* h, const char* what, int words, int key_bits,
   return host_c ? download (h, c2, nw, *host_c) : B200TSDF_OK;
 }
 
+bool create_events (Event* e, int n, unsigned flags)
+{
+  for (int i = 0; i < n; ++i)
+    if (cudaEventCreateWithFlags (&e[i].x, flags) != cudaSuccess) return false;
+  return true;
+}
+
 } // namespace
+
+b200tsdf::~b200tsdf ()
+{
+  drop_batch_graphs (this);
+  delete pack_pool;
+  std::free (mesh_v); std::free (mesh_c); std::free (leaf_xyz); std::free (leaf_ijk);
+}
 
 extern "C" {
 
@@ -1028,40 +1090,27 @@ int b200tsdf_create (const b200tsdf_config* cfg, b200tsdf_t** out)
   if (const char* e = std::getenv ("B200TSDF_HOST_PACK")) h->host_pack = std::atoi (e) != 0 ? 1 : 0;
   if (const char* e = std::getenv ("B200TSDF_PACK_THREADS")) { const int v = std::atoi (e); if (v >= 1 && v <= 256) h->pack_threads = v; }
   if (h->device < 0 || h->device >= ndev) { delete h; return B200TSDF_EINVAL; }
+  const unsigned nt = cudaEventDisableTiming;
   bool ok = cudaSetDevice (h->device) == cudaSuccess
          && cudaDeviceGetAttribute (&h->sm_count, cudaDevAttrMultiProcessorCount, h->device) == cudaSuccess
-         && cudaStreamCreateWithFlags (&h->stream, cudaStreamNonBlocking) == cudaSuccess
-         && cudaStreamCreateWithFlags (&h->copy_stream, cudaStreamNonBlocking) == cudaSuccess
-         && cudaStreamCreateWithFlags (&h->gather_stream, cudaStreamNonBlocking) == cudaSuccess
-         && cudaMalloc (&h->d_err, sizeof (int)) == cudaSuccess
-         && cudaMalloc (&h->d_count, 64 * sizeof (int)) == cudaSuccess
-         && cudaMalloc (&h->d_stats, ST_TOTAL * sizeof (unsigned long long)) == cudaSuccess
-         && cudaMalloc (&h->d_params, sizeof (Params)) == cudaSuccess
-         && cudaHostAlloc (&h->h_err, sizeof (int), cudaHostAllocDefault) == cudaSuccess
-         && cudaMalloc (&h->d_ring, FRAME_RING * sizeof (FrameRec)) == cudaSuccess
-         && cudaHostAlloc (&h->h_ring, FRAME_RING * sizeof (FrameRec), cudaHostAllocDefault) == cudaSuccess
-         && cudaEventCreateWithFlags (&h->ev_ring[0], cudaEventDisableTiming) == cudaSuccess
-         && cudaEventCreateWithFlags (&h->ev_ring[1], cudaEventDisableTiming) == cudaSuccess
-         && cudaMalloc (&h->d_bring, 2 * BRING_SPAN * sizeof (FrameRec)) == cudaSuccess
-         && cudaHostAlloc (&h->h_bring, (size_t) BATCH_SEGS * BRING_SPAN * sizeof (FrameRec), cudaHostAllocDefault) == cudaSuccess
-         && cudaEventCreateWithFlags (&h->ev_rows_done[0], cudaEventDisableTiming) == cudaSuccess
-         && cudaEventCreateWithFlags (&h->ev_rows_done[1], cudaEventDisableTiming) == cudaSuccess;
-  for (int i = 0; ok && i < BATCH_SEGS; ++i) ok = cudaEventCreateWithFlags (&h->ev_bring[i], cudaEventDisableTiming) == cudaSuccess;
-  for (int i = 0; ok && i < 2; ++i) ok = cudaEventCreateWithFlags (&h->ev_half_done[i], cudaEventDisableTiming) == cudaSuccess;
-  for (int i = 0; ok && i < 2; ++i)
-    ok = cudaEventCreateWithFlags (&h->ev_copied[i], cudaEventDisableTiming) == cudaSuccess
-      && cudaEventCreateWithFlags (&h->ev_consumed[i], cudaEventDisableTiming) == cudaSuccess;
-  ok = ok && cudaEventCreate (&h->ev_t0) == cudaSuccess && cudaEventCreate (&h->ev_t1) == cudaSuccess
-          && cudaEventCreate (&h->ev_p0) == cudaSuccess && cudaEventCreate (&h->ev_p1) == cudaSuccess;
-  for (int i = 0; ok && i < 64; ++i) ok = cudaEventCreateWithFlags (&h->ev_rows_ready[i / 32][i % 32], cudaEventDisableTiming) == cudaSuccess
-                                          && cudaEventCreateWithFlags (&h->ev_rows_up[i / 32][i % 32], cudaEventDisableTiming) == cudaSuccess;
-  for (int i = 0; ok && i < KRING; ++i)
-    ok = cudaEventCreate (&h->kring[i][0]) == cudaSuccess && cudaEventCreate (&h->kring[i][1]) == cudaSuccess;
-  if (ok) *h->h_err = 0;
-  if (ok) { cudaMemset (h->d_err, 0, sizeof (int)); cudaMemset (h->d_stats, 0, ST_TOTAL * sizeof (unsigned long long)); }
+         && cudaStreamCreateWithFlags (&h->stream.x, cudaStreamNonBlocking) == cudaSuccess
+         && cudaStreamCreateWithFlags (&h->copy_stream.x, cudaStreamNonBlocking) == cudaSuccess
+         && cudaStreamCreateWithFlags (&h->gather_stream.x, cudaStreamNonBlocking) == cudaSuccess
+         && !h->d_err.grow (1) && !h->d_count.grow (64) && !h->d_stats.grow (ST_TOTAL) && !h->d_params.grow (1)
+         && !h->d_ring.grow (FRAME_RING) && !h->d_bring.grow (2 * BRING_SPAN) && !h->d_rrec.grow (RENDER_CHUNK)
+         && !h->h_err.alloc (1) && !h->h_ring.alloc (FRAME_RING) && !h->h_bring.alloc ((size_t) BATCH_SEGS * BRING_SPAN)
+         && !h->h_rrec.alloc ((size_t) RENDER_SEGS * RENDER_CHUNK)
+         && create_events (h->ev_ring, 2, nt) && create_events (h->ev_rows_done, 2, nt) && create_events (h->ev_bring, BATCH_SEGS, nt)
+         && create_events (h->ev_half_done, 2, nt) && create_events (h->ev_copied, 2, nt) && create_events (h->ev_consumed, 2, nt)
+         && create_events (h->ev_rrec, RENDER_SEGS, nt) && create_events (&h->ev_rows_ready[0][0], 64, nt) && create_events (&h->ev_rows_up[0][0], 64, nt)
+         && create_events (&h->ev_t0, 1, cudaEventDefault) && create_events (&h->ev_t1, 1, cudaEventDefault)
+         && create_events (&h->ev_p0, 1, cudaEventDefault) && create_events (&h->ev_p1, 1, cudaEventDefault)
+         && create_events (&h->kring[0][0], 2 * KRING, cudaEventDefault);
+  if (!ok) { delete h; return B200TSDF_ECUDA; }
+  *h->h_err = 0;
+  cudaMemset (h->d_err, 0, sizeof (int)); cudaMemset (h->d_stats, 0, ST_TOTAL * sizeof (unsigned long long));
   // the depth-first general path recurses up to (L - C + 1) levels
-  if (ok) cudaDeviceSetLimit (cudaLimitStackSize, 16384);
-  if (!ok) { b200tsdf_destroy (h); return B200TSDF_ECUDA; }
+  cudaDeviceSetLimit (cudaLimitStackSize, 16384);
   *out = h;
   return B200TSDF_OK;
 }
@@ -1073,37 +1122,7 @@ void b200tsdf_destroy (b200tsdf_t* h)
   if (h->stream) cudaStreamSynchronize (h->stream);
   if (h->copy_stream) cudaStreamSynchronize (h->copy_stream);
   if (h->gather_stream) cudaStreamSynchronize (h->gather_stream);
-  free_volume (h);
-  cudaFree (h->d_err); cudaFree (h->d_count); cudaFree (h->d_stats); cudaFree (h->d_culled); cudaFree (h->d_pix); cudaFree (h->d_scratch);
-  cudaFree (h->d_dbg); if (h->h_err) cudaFreeHost (h->h_err);
-  cudaFree (h->d_params); cudaFree (h->d_ring); if (h->h_ring) cudaFreeHost (h->h_ring);
-  for (int i = 0; i < 2; ++i) if (h->ev_ring[i]) cudaEventDestroy (h->ev_ring[i]);
-  drop_batch_graphs (h);
   comm_release (h);
-  delete h->pack_pool; h->pack_pool = nullptr;
-  for (int i = 0; i < 2; ++i)
-  {
-    cudaFree (h->d_rows_raw[i]); cudaFree (h->d_rows_full[i]);
-    h->h_pack[i].release (); h->h_fpack[i].release ();
-    for (int k = 0; k < 32; ++k) { if (h->ev_rows_ready[i][k]) cudaEventDestroy (h->ev_rows_ready[i][k]); if (h->ev_rows_up[i][k]) cudaEventDestroy (h->ev_rows_up[i][k]); }
-    if (h->ev_rows_done[i]) cudaEventDestroy (h->ev_rows_done[i]);
-  }
-  cudaFree (h->d_bring); if (h->h_bring) cudaFreeHost (h->h_bring);
-  cudaFree (h->d_org);
-  cudaFree (h->d_rrec); if (h->h_rrec) cudaFreeHost (h->h_rrec);
-  for (int i = 0; i < RENDER_SEGS; ++i) if (h->ev_rrec[i]) cudaEventDestroy (h->ev_rrec[i]);
-  for (int i = 0; i < BATCH_SEGS; ++i) if (h->ev_bring[i]) cudaEventDestroy (h->ev_bring[i]);
-  for (int i = 0; i < 2; ++i) if (h->ev_half_done[i]) cudaEventDestroy (h->ev_half_done[i]);
-  cudaFree (h->d_frame[0]); cudaFree (h->d_frame[1]); cudaFree (h->q_mem); cudaFree (h->d_blist); cudaFree (h->d_cellq); cudaFree (h->d_superq); cudaFree (h->d_celltop);
-  cudaFree (h->d_fold); cudaFree (h->d_q1);
-  for (int i = 0; i < 2; ++i) { if (h->ev_copied[i]) cudaEventDestroy (h->ev_copied[i]); if (h->ev_consumed[i]) cudaEventDestroy (h->ev_consumed[i]); }
-  if (h->ev_t0) cudaEventDestroy (h->ev_t0); if (h->ev_t1) cudaEventDestroy (h->ev_t1);
-  if (h->ev_p0) cudaEventDestroy (h->ev_p0); if (h->ev_p1) cudaEventDestroy (h->ev_p1);
-  for (int i = 0; i < KRING; ++i) { if (h->kring[i][0]) cudaEventDestroy (h->kring[i][0]); if (h->kring[i][1]) cudaEventDestroy (h->kring[i][1]); }
-  if (h->stream) cudaStreamDestroy (h->stream);
-  if (h->copy_stream) cudaStreamDestroy (h->copy_stream);
-  if (h->gather_stream) cudaStreamDestroy (h->gather_stream);
-  std::free (h->mesh_v); std::free (h->mesh_c); std::free (h->leaf_xyz); std::free (h->leaf_ijk);
   delete h;
 }
 
@@ -1129,6 +1148,32 @@ int b200tsdf_get_config (const b200tsdf_t* h, b200tsdf_config* cfg)
 }
 
 // ---- reset (tsdf_volume_octree.cpp:201-219, Octree::init octree.cpp:584-599) --------------------
+// The integrate route of configuration np: which kernels fuse a frame, and the capacities of their work queues (Q.cap; reset
+// installs the queues once their memory is allocated)
+static void choose_route (b200tsdf* h, const Params& np, int debug_flags)
+{
+  // work queues for levels C .. B = L-3 (fast path needs the block-root level at or below the coarse depth)
+  // the brick kernels divide with div_recip / div_with, which equal __fdiv_rn only inside Params::exact_div_ok; other
+  // truncation limits and weight caps are fused by the general depth-first kernel, which uses the IEEE division
+  const int Bl = np.L - 3;
+  h->fast_path = (Bl >= np.C) && !np.track_var && !np.color_norm && !(debug_flags & 1) && np.exact_div_ok && (Bl - np.C + 1 <= MAX_QLEVELS);
+  h->q_levels = h->fast_path ? (Bl - np.C + 1) : 0;
+  h->Q = Queues {};
+  for (int i = 0; i < h->q_levels; ++i) h->Q.cap[i] = np.C + i >= 7 ? 1 << 21 : 1 << (3 * (np.C + i));
+  // supercell path (k_celltop_down / k_bricks / k_celltop_up, brick_kernels.cuh): needs tier-1 bricks (T >= 2), whose roots sit
+  // at level SL = L - 6.  Coarse levels above SL are swept by k_upper_*; coarse cells below SL are handled inside the brick.
+  h->sl = np.L - 6;
+  h->nup = std::max (0, h->sl - np.C);
+  h->super_static = 0;
+  h->top_path = h->fast_path && np.T >= 2 && h->sl >= 0 && !(debug_flags & 2);
+  if (h->top_path && np.C > h->sl)
+  {
+    // every tier-1 root is a supercell; they must be the root-array nodes (T == 2) and fit the per-cell scratch
+    if (np.Rtop != h->sl || h->sl > 4) h->top_path = false;
+    else h->super_static = 1 << (3 * h->sl);
+  }
+}
+
 int b200tsdf_reset (b200tsdf_t* h)
 {
   if (!h) return B200TSDF_EINVAL;
@@ -1137,137 +1182,50 @@ int b200tsdf_reset (b200tsdf_t* h)
   Params np = h->p;
   size_t pool = 0, root_n = 0;
   if (const char* msg = derive_params (c, np, pool, root_n)) return h->fail (B200TSDF_EINVAL, msg);
-  bool color = np.color != 0, var = np.track_var != 0, norm = np.color_norm != 0;
-  int C = np.C, Rtop = np.Rtop;
+  const bool color = np.color != 0, var = np.track_var != 0, norm = np.color_norm != 0;
 
+  // from here on a failure leaves the handle without a volume until a reset succeeds
+  h->has_volume = false;
   CK (cudaStreamSynchronize (h->stream));
   CK (cudaStreamSynchronize (h->copy_stream));
   drop_batch_graphs (h);                                   // captured launches carry the old configuration
-  cudaFree (h->d_org); h->d_org = nullptr;                 // (sized by the old image size; the graphs that used it are gone)
+  h->d_org.release ();                                     // (sized by the old image size; the graphs that used it are gone)
   for (int i = 0; i < BATCH_SEGS; ++i) h->bring_used[i] = false;
   h->half_used[0] = h->half_used[1] = false;
-  if (pool != h->pool || root_n != h->root_n || color != h->alloc_color || var != h->alloc_var || norm != h->alloc_norm)
+  choose_route (h, np, c.debug_flags);
+  const bool fold = h->top_path && h->sl == np.C;          // publishes_folds of the new route
+
+  Volume& v = h->vol;
+  if (pool != v.pool || root_n != v.root_n || color != v.color || var != v.var || norm != v.norm)
   {
-    h->has_volume = false;                                 // a failed allocation below must not leave a half-built volume usable
-    free_volume (h);
-    CK (cudaMalloc (&h->p.keys, pool * sizeof (uint64_t)));
-    CK (cudaMalloc (&h->p.nodes, pool * BRICK_NODES * sizeof (float2)));
-    CK (cudaMalloc (&h->p.split, pool * BRICK_SPLIT_WORDS * sizeof (uint32_t)));
-    CK (cudaMalloc (&h->p.work, pool));
-    if (color) CK (cudaMalloc (&h->p.rgb, pool * BRICK_NODES * sizeof (uchar4)));
-    if (var) { CK (cudaMalloc (&h->p.M, pool * BRICK_NODES * sizeof (float))); CK (cudaMalloc (&h->p.ns, pool * BRICK_NODES * sizeof (int))); }
-    CK (cudaMalloc (&h->p.root_dw, root_n * sizeof (float2)));
-    CK (cudaMalloc (&h->p.root_split, ((root_n + 31) / 32) * sizeof (uint32_t)));
-    if (color) CK (cudaMalloc (&h->p.root_rgb, root_n * sizeof (uchar4)));
-    if (norm) { CK (cudaMalloc (&h->p.rgbn, pool * BRICK_NODES * sizeof (float4))); CK (cudaMalloc (&h->p.root_rgbn, root_n * sizeof (float4))); }
-    if (var) { CK (cudaMalloc (&h->p.root_M, root_n * sizeof (float))); CK (cudaMalloc (&h->p.root_ns, root_n * sizeof (int))); }
-    h->pool = pool; h->root_n = root_n; h->alloc_color = color; h->alloc_var = var; h->alloc_norm = norm;
+    v = {};                                                // (the old storage is freed before the new one is allocated)
+    const size_t nn = pool * BRICK_NODES;
+    if (v.keys.grow (pool) || v.nodes.grow (nn) || v.split.grow (pool * BRICK_SPLIT_WORDS) || v.work.grow (pool)
+        || (color && v.rgb.grow (nn)) || (var && (v.M.grow (nn) || v.ns.grow (nn)))
+        || v.root_dw.grow (root_n) || v.root_split.grow ((root_n + 31) / 32) || (color && v.root_rgb.grow (root_n))
+        || (norm && (v.rgbn.grow (nn) || v.root_rgbn.grow (root_n))) || (var && (v.root_M.grow (root_n) || v.root_ns.grow (root_n))))
+      return alloc_failed (h, "volume storage");
+    v.pool = pool; v.root_n = root_n; v.color = color; v.var = var; v.norm = norm;
   }
-  size_t ncells = (size_t) 1 << (3 * C);
-  if (ncells > h->culled_cap)
-  {
-    cudaFree (h->d_culled); h->d_culled = nullptr;
-    CK (cudaMalloc (&h->d_culled, ncells * sizeof (int)));
-    h->culled_cap = ncells;
-  }
-  const size_t pix_bytes = 2 * (size_t) np.width * np.height * (color ? 8 : 4);   // two planes alternate by counter set (frame_plane)
-  if (pix_bytes > h->pix_cap)
-  {
-    h->has_volume = false;                                 // the frames' launches need the plane
-    cudaFree (h->d_pix); h->d_pix = nullptr; h->pix_cap = 0; h->p.pix = nullptr;
-    CK (cudaMalloc (&h->d_pix, pix_bytes));
-    h->pix_cap = pix_bytes;
-  }
-  {
-    // work queues for levels C .. B = L-3 (fast path needs the block-root level at or below the coarse depth)
-    // the brick kernels divide with div_recip / div_with, which equal __fdiv_rn only inside Params::exact_div_ok; other
-    // truncation limits and weight caps are fused by the general depth-first kernel, which uses the IEEE division
-    int Bl = np.L - 3;
-    h->force_general = c.debug_flags & 1;
-    h->fast_path = (Bl >= np.C) && !var && !np.color_norm && !h->force_general && np.exact_div_ok && (Bl - np.C + 1 <= MAX_QLEVELS);
-    h->q_levels = h->fast_path ? (Bl - np.C + 1) : 0;
-    size_t total = 0; size_t caps[MAX_QLEVELS] = {};
-    for (int i = 0; i < h->q_levels; ++i)
-    {
-      int lv = np.C + i;
-      size_t full = lv >= 7 ? ((size_t) 1 << 21) : ((size_t) 1 << (3 * lv));
-      caps[i] = std::min (full, (size_t) 1 << 21);
-      total += caps[i];
-    }
-    if (total > h->q_mem_cap)
-    {
-      cudaFree (h->q_mem); h->q_mem = nullptr; h->q_mem_cap = 0;
-      CK (cudaMalloc (&h->q_mem, total * sizeof (QNode)));
-      h->q_mem_cap = total;
-    }
-    size_t off = 0;
-    for (int i = 0; i < MAX_QLEVELS; ++i) { h->Q.q[i] = nullptr; h->Q.cap[i] = 0; }
-    for (int i = 0; i < h->q_levels; ++i) { h->Q.q[i] = h->q_mem + off; h->Q.cap[i] = (int) caps[i]; off += caps[i]; }
-    h->Q.n = h->d_count;
-    // supercell path (k_celltop_down / k_bricks / k_celltop_up, brick_kernels.cuh): needs tier-1 bricks (T >= 2), whose roots sit
-    // at level SL = L - 6.  Coarse levels above SL are swept by k_upper_*; coarse cells below SL are handled inside the brick.
-    h->sl = np.L - 6;
-    h->nup = std::max (0, h->sl - np.C);
-    h->super_static = 0;
-    h->top_path = h->fast_path && np.T >= 2 && h->sl >= 0 && !(c.debug_flags & 2);
-    if (h->top_path && np.C > h->sl)
-    {
-      // every tier-1 root is a supercell; they must be the root-array nodes (T == 2) and fit the per-cell scratch
-      if (np.Rtop != h->sl || h->sl > 4) h->top_path = false;
-      else h->super_static = 1 << (3 * h->sl);
-    }
-    if (h->top_path)
-    {
-      h->cell_cap = 16384;
-      size_t need = (size_t) h->cell_cap * 585;
-      if (need > h->cellq_cap)
-      {
-        cudaFree (h->d_cellq); cudaFree (h->d_celltop); h->d_cellq = nullptr; h->d_celltop = nullptr; h->cellq_cap = 0;
-        CK (cudaMalloc (&h->d_cellq, need * sizeof (QNode)));
-        CK (cudaMalloc (&h->d_celltop, (size_t) h->cell_cap * sizeof (CellTop)));
-        h->cellq_cap = need;
-      }
-      if (h->super_static && !h->d_superq) CK (cudaMalloc (&h->d_superq, 4096 * sizeof (QNode)));
-    }
-    if (h->top_path && h->sl == np.C)
-    {
-      // the per-supercell gate of k_front (FoldState): fold marks over the coarse cells, and a second level-C queue
-      const size_t fw = fold_words (np.C);
-      if (fw > h->fold_cap)
-      {
-        cudaFree (h->d_fold); h->d_fold = nullptr; h->fold_cap = 0;
-        CK (cudaMalloc (&h->d_fold, fw * sizeof (uint32_t)));
-        h->fold_cap = fw;
-      }
-      if ((size_t) h->Q.cap[0] > h->q1_cap)
-      {
-        cudaFree (h->d_q1); h->d_q1 = nullptr; h->q1_cap = 0;
-        CK (cudaMalloc (&h->d_q1, (size_t) h->Q.cap[0] * sizeof (QNode)));
-        h->q1_cap = h->Q.cap[0];
-      }
-    }
-    size_t bl = h->q_levels ? caps[h->q_levels - 1] : 0;
-    if (h->top_path) bl = std::max (bl, (size_t) h->cell_cap * 512);
-    if (bl > h->blist_cap)
-    {
-      cudaFree (h->d_blist); h->d_blist = nullptr; h->blist_cap = 0;
-      CK (cudaMalloc (&h->d_blist, bl * BL_CLASSES * sizeof (int)));          // one list per work class
-      h->blist_cap = bl;
-    }
-  }
+  size_t q_total = 0;
+  for (int i = 0; i < h->q_levels; ++i) q_total += (size_t) h->Q.cap[i];
+  size_t bl = h->q_levels ? (size_t) h->Q.cap[h->q_levels - 1] : 0;
+  if (h->top_path) bl = std::max (bl, (size_t) CELL_CAP * 512);
+  if (h->d_culled.grow ((size_t) 1 << (3 * np.C))
+      || h->d_pix.grow (2 * (size_t) np.width * np.height * (color ? 2 : 1))    // two planes alternate by counter set (frame_plane)
+      || h->q_mem.grow (q_total)
+      || h->d_blist.grow (bl * BL_CLASSES)                                      // one list per work class
+      || (h->top_path && (h->d_cellq.grow ((size_t) CELL_CAP * 585) || h->d_celltop.grow (CELL_CAP)))
+      || (h->super_static && h->d_superq.grow (4096))
+      || (fold && (h->d_fold.grow (fold_words (np.C)) || h->d_q1.grow ((size_t) h->Q.cap[0]))))
+    return alloc_failed (h, "work queues");
+
+  // install the configuration
   Params& p = h->p;
-  {
-    // keep the storage pointers, take every scalar from the derived set
-    Params st = p;
-    p = np;
-    p.work = st.work;
-    p.keys = st.keys; p.nodes = st.nodes; p.split = st.split; p.rgb = st.rgb; p.M = st.M; p.ns = st.ns;
-    p.root_dw = st.root_dw; p.root_split = st.root_split; p.root_rgb = st.root_rgb; p.root_M = st.root_M; p.root_ns = st.root_ns;
-    p.rgbn = st.rgbn; p.root_rgbn = st.root_rgbn;
-  }
-  p.err = h->d_err;
-  p.pix = h->d_pix;
-  p.dbg = h->d_dbg;
+  p = np;
+  h->storage_into (p);
+  h->Q.n = h->d_count;
+  for (size_t i = 0, off = 0; i < (size_t) h->q_levels; off += (size_t) h->Q.cap[i++]) h->Q.q[i] = h->q_mem + off;
   CK (cudaMemcpyAsync (h->d_params, &p, sizeof (Params), cudaMemcpyHostToDevice, h->stream));
   CK (cudaStreamSynchronize (h->stream));                            // (&p is host memory that may change after reset)
   // fresh state everywhere (OctreeNode ctor: d=-1, w=0; octree.h:71-74)
@@ -1287,18 +1245,18 @@ int b200tsdf_reset (b200tsdf_t* h)
   *h->h_err = 0;
   CK (cudaMemsetAsync (h->d_count, 0, 64 * sizeof (int), s));
   h->count_set = 0;
-  if (h->d_fold) CK (cudaMemsetAsync (h->d_fold, 0, h->fold_cap * sizeof (uint32_t), s));
+  if (h->d_fold) CK (cudaMemsetAsync (h->d_fold, 0, h->d_fold.cap * sizeof (uint32_t), s));
   h->fold_prev = false;
   CK (cudaMemsetAsync (h->d_stats, 0, ST_TOTAL * sizeof (unsigned long long), s));
   h->kring_pending = 0; h->kring_head = 0;
-  if (Rtop < C) k_insert_top_bricks<<<(unsigned) ((root_n + 127) / 128), 128, 0, s>>> (p);
+  if (np.Rtop < np.C) k_insert_top_bricks<<<(unsigned) ((root_n + 127) / 128), 128, 0, s>>> (p);
   if (h->top_path && h->super_static) k_build_superq<<<(h->super_static + 127) / 128, 128, 0, s>>> (p, h->d_superq, h->super_static);
   CK (cudaGetLastError ());
   h->cfg = c;
-  h->has_volume = true;
   h->frame_no = 0;
   h->timed = false;
   h->is_empty = true;
+  h->has_volume = true;
   return check_device_err (h);
 }
 
@@ -1339,7 +1297,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, boo
   // on the route that publishes fold marks, frames alternate between two cell queues (k_front fills the next frame's while
   // this frame's k_celltop_up still reads its own); other routes use Q.q[0] for both counter sets
   const bool pub = publishes_folds (h);
-  uint32_t* const fold = pub ? h->d_fold : nullptr;
+  uint32_t* const fold = pub ? h->d_fold.p : nullptr;
   QNode* const q1 = pub ? h->d_q1 : h->Q.q[0];
   {
     const int cull_blocks = (ncells + 255) / 256;
@@ -1365,7 +1323,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, boo
       QNode* cells = h->super_static ? h->d_superq : h->Q.q[h->nup];
       const int qslot = h->super_static ? -1 : h->nup;
       auto kd = p.color ? k_celltop_down<true> : k_celltop_down<false>;
-      CK (launch_pdl (kd, dim3 (h->sm_count * 4), dim3 (TOP_THREADS), s, p, d_rec, cells, pub ? q1 : cells, h->d_count, h->d_cellq, h->d_celltop, h->cell_cap, h->d_blist, (int) h->blist_cap, h->d_stats, h->sl, qslot, h->super_static, fold));
+      CK (launch_pdl (kd, dim3 (h->sm_count * 4), dim3 (TOP_THREADS), s, p, d_rec, cells, pub ? q1 : cells, h->d_count, h->d_cellq, h->d_celltop, CELL_CAP, h->d_blist, h->blist_cap (), h->d_stats, h->sl, qslot, h->super_static, fold));
       h->launches++;
       bq = h->d_cellq;
     }
@@ -1379,8 +1337,8 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, boo
     {
       auto kb = p.color ? k_bricks<true> : k_bricks<false>;
       const dim3 g (h->sm_count * BD_CTAS), b (BD_WARPS * 32);
-      if (h->top_path) CK (launch_pdl (kb, g, b, s, p, (const Params*) h->d_params, d_rec, bq, (const int*) h->d_blist, (int) h->blist_cap, h->d_count, h->d_stats, p.L - 3));
-      else kb<<<g, b, 0, s>>> (p, h->d_params, d_rec, bq, h->d_blist, (int) h->blist_cap, h->d_count, h->d_stats, p.L - 3);
+      if (h->top_path) CK (launch_pdl (kb, g, b, s, p, (const Params*) h->d_params, d_rec, bq, (const int*) h->d_blist, h->blist_cap (), h->d_count, h->d_stats, p.L - 3));
+      else kb<<<g, b, 0, s>>> (p, h->d_params, d_rec, bq, h->d_blist, h->blist_cap (), h->d_count, h->d_stats, p.L - 3);
     }
     if (kr >= 0) CK (cudaEventRecord (h->kring[kr][1], s));
     h->launches++;
@@ -1389,7 +1347,7 @@ static int launch_frame (b200tsdf* h, cudaStream_t s, const FrameRec* d_rec, boo
       QNode* cells = h->super_static ? h->d_superq : h->Q.q[h->nup];
       const int qslot = h->super_static ? -1 : h->nup;
       auto ku = p.color ? k_celltop_up<true> : k_celltop_up<false>;
-      CK (launch_pdl (ku, dim3 (h->sm_count), dim3 (128), s, p, d_rec, cells, pub ? q1 : cells, (const int*) h->d_count, (const QNode*) h->d_cellq, (const CellTop*) h->d_celltop, h->cell_cap, h->d_stats, h->sl, qslot, h->super_static, fold));
+      CK (launch_pdl (ku, dim3 (h->sm_count), dim3 (128), s, p, d_rec, cells, pub ? q1 : cells, (const int*) h->d_count, (const QNode*) h->d_cellq, (const CellTop*) h->d_celltop, CELL_CAP, h->d_stats, h->sl, qslot, h->super_static, fold));
       h->launches++;
       for (int li = h->nup - 1; li >= 0; --li) { k_upper_up<<<h->sm_count * 2, 128, 0, s>>> (p, d_rec, h->Q, li, h->d_stats); h->launches++; }
     }
@@ -1502,14 +1460,12 @@ static int batch_records (b200tsdf* h, int m, const void* const* d_points, size_
 }
 // the organised images of the unorganised batch path (layout: keys HALF*npix*8 | filled counters HALF*8 | images HALF*npix*16)
 static size_t org_npix (const b200tsdf* h) { return (size_t) h->cfg.image_width * h->cfg.image_height; }
-static unsigned long long* org_keys (const b200tsdf* h) { return reinterpret_cast<unsigned long long*> (h->d_org); }
+static unsigned long long* org_keys (const b200tsdf* h) { return reinterpret_cast<unsigned long long*> (h->d_org.p); }
 static unsigned long long* org_filled (const b200tsdf* h) { return org_keys (h) + ORG_MAX_FRAMES * org_npix (h); }
 static unsigned char* org_images (const b200tsdf* h) { return h->d_org + ORG_MAX_FRAMES * org_npix (h) * 8 + 256; }
 static int org_buffers (b200tsdf* h)
 {
-  if (h->d_org) return B200TSDF_OK;
-  const size_t bytes = ORG_MAX_FRAMES * org_npix (h) * (8 + 16) + 256;
-  if (cudaMalloc (&h->d_org, bytes) != cudaSuccess) { h->d_org = nullptr; return alloc_failed (h, "organised images of an unorganised batch"); }
+  if (h->d_org.grow (ORG_MAX_FRAMES * org_npix (h) * (8 + 16) + 256)) return alloc_failed (h, "organised images of an unorganised batch");
   return B200TSDF_OK;
 }
 
@@ -1632,24 +1588,23 @@ static int integrate_host (b200tsdf* h, const void* points, size_t stride, int x
   const bool hpack = host_pack_wanted (h, stride, h->comm ? h->comm_size : 1);
   const size_t npts = (size_t) width * height;
   const size_t bytes = hpack ? npts * 16 : npts * stride;
-  if (bytes > h->frame_cap || (hpack && !h->h_fpack[0].p))
+  const size_t frame_cap = std::min (h->d_frame[0].cap, h->d_frame[1].cap);
+  if (bytes > frame_cap || (hpack && !h->h_fpack[0].p))
   {
     CK (cudaStreamSynchronize (h->stream)); CK (cudaStreamSynchronize (h->copy_stream));
-    const size_t cap = std::max (bytes, h->frame_cap);
+    const size_t cap = std::max (bytes, frame_cap);
     for (int i = 0; i < 2; ++i)
     {
-      cudaFree (h->d_frame[i]); h->d_frame[i] = nullptr; CK (cudaMalloc (&h->d_frame[i], cap));
+      CK (h->d_frame[i].grow (cap));
       h->h_fpack[i].release ();
       if (hpack && h->h_fpack[i].alloc (cap))
       {
         // no pinned staging to be had on this system: upload the points as they are from now on
         h->host_pack = 0;
-        for (int k = 0; k < 2; ++k) h->h_fpack[k].release ();
-        h->frame_cap = 0;                                  // (d_frame[] is re-sized by the unpacked path)
+        for (int k = 0; k < 2; ++k) { h->h_fpack[k].release (); h->d_frame[k].release (); }   // (re-sized by the unpacked path)
         return integrate_host (h, points, stride, xyz_off, rgba_off, width, height, pose, wait_copy);
       }
     }
-    h->frame_cap = cap;
     h->frame_no = 0;
   }
   // double-buffered upload on the copy stream: frame i+1 crosses PCIe while frame i is fused
@@ -1862,12 +1817,12 @@ int b200tsdf_get_stats (b200tsdf_t* h, b200tsdf_stats* s)
   s->n_block_visits = (int64_t) (st[ST_BLOCKS] - st[ST_N + ST_BLOCKS]);
   s->reserved = 0; s->n_bail = 0; s->n_slow_visits = 0;   // (kept for the layout; always 0)
   s->n_culled_cells = cnt[0];
-  s->pool_capacity = (int64_t) h->pool;
+  s->pool_capacity = (int64_t) h->vol.pool;
   s->coarse_level = h->p.C; s->finest_level = h->p.L; s->tiers = h->p.T;
   // allocated bricks (no allocation, no list: this call sits in measured loops)
   int* d_n = h->d_count + 40;
   CK (cudaMemsetAsync (d_n, 0, sizeof (int), h->stream));
-  k_count_bricks<<<(unsigned) ((h->pool + 255) / 256), 256, 0, h->stream>>> (h->p, d_n);
+  k_count_bricks<<<(unsigned) ((h->vol.pool + 255) / 256), 256, 0, h->stream>>> (h->p, d_n);
   int nb = 0;
   CK (cudaMemcpyAsync (&nb, d_n, sizeof (int), cudaMemcpyDeviceToHost, h->stream));
   CK (cudaStreamSynchronize (h->stream));
@@ -1912,7 +1867,7 @@ int b200tsdf_query (b200tsdf_t* h, const float* xyz, int n, int what, int mode,
   cudaSetDevice (h->device);
   // one scratch block: xyz (12n) | val (4n) | grad (12n) | hess (36n) | ok (n)
   { int rc = h->scratch ((size_t) n * 65 + 64); if (rc) return rc; }
-  float* d_xyz = (float*) h->d_scratch;
+  float* d_xyz = (float*) h->d_scratch.p;
   float* d_val = d_xyz + (size_t) 3 * n;
   float* d_grad = d_val + n;
   float* d_hess = d_grad + (size_t) 3 * n;
@@ -1954,7 +1909,7 @@ int b200tsdf_interpolate (b200tsdf_t* h, const float* xyz, int n, float* val, ui
   if (n == 0) return B200TSDF_OK;
   cudaSetDevice (h->device);
   { int rc = h->scratch ((size_t) n * 17 + 64); if (rc) return rc; }
-  float* d_xyz = (float*) h->d_scratch;
+  float* d_xyz = (float*) h->d_scratch.p;
   float* d_val = d_xyz + (size_t) 3 * n;
   unsigned char* d_ok = (unsigned char*) (d_val + n);
   cudaStream_t s = h->stream;
@@ -2007,7 +1962,7 @@ int b200tsdf_containing_voxels (b200tsdf_t* h, const float* xyz, size_t n, float
   cudaSetDevice (h->device);
   // one scratch block: xyz (12 n) | records (44 n)
   { int rc = h->scratch (n * (12 + sizeof (b200tsdf_voxel)) + 64); if (rc) return rc; }
-  float* d_xyz = (float*) h->d_scratch;
+  float* d_xyz = (float*) h->d_scratch.p;
   b200tsdf_voxel* d_out = (b200tsdf_voxel*) (d_xyz + 3 * n);
   cudaStream_t s = h->stream;
   CK (cudaMemcpyAsync (d_xyz, xyz, n * 12, cudaMemcpyHostToDevice, s));
@@ -2094,7 +2049,7 @@ int b200tsdf_set_containing_voxels (b200tsdf_t* h, const float* xyz, size_t n, f
   // one scratch block: xyz (12 n) | d (4 n) | w (4 n) | status (n) | the work space of edit_batch (16-byte aligned)
   const size_t in_bytes = (n * 21 + 15) & ~(size_t) 15;
   { int rc = h->scratch (in_bytes + edit_work_bytes (n)); if (rc) return rc; }
-  float* d_xyz = (float*) h->d_scratch;
+  float* d_xyz = (float*) h->d_scratch.p;
   float* d_d = d_xyz + 3 * n;
   float* d_w = d_d + n;
   uint8_t* d_status = (uint8_t*) (d_w + n);
@@ -2152,12 +2107,6 @@ static int render_enqueue (b200tsdf* h, int n, const double* poses, int downsamp
                            int xyz_off, int normal_off, unsigned char* d_rgb)
 {
   cudaStream_t s = h->stream;
-  if (!h->d_rrec)
-  {
-    CK (cudaMalloc (&h->d_rrec, RENDER_CHUNK * sizeof (RenderParams)));
-    CK (cudaHostAlloc (&h->h_rrec, (size_t) RENDER_SEGS * RENDER_CHUNK * sizeof (RenderParams), cudaHostAllocDefault));
-    for (int i = 0; i < RENDER_SEGS; ++i) CK (cudaEventCreateWithFlags (&h->ev_rrec[i], cudaEventDisableTiming));
-  }
   const Params& p = h->p;
   const int W = p.width / downsample, H = p.height / downsample;
   const size_t npix = (size_t) W * H;
@@ -2238,7 +2187,7 @@ static int marching_cubes (b200tsdf* h, float w_min, int color_mode, const Sort&
   int* list = nullptr;
   const int nb = list_bricks (h, list);
   if (nb < 0) return nb;
-  const unsigned bgrid = (unsigned) (((size_t) nb * 32 + 127) / 128), rgrid = (unsigned) ((h->root_n + 127) / 128);
+  const unsigned bgrid = (unsigned) (((size_t) nb * 32 + 127) / 128), rgrid = (unsigned) ((h->vol.root_n + 127) / 128);
   auto launch = [&] (auto emit, unsigned long long* total, unsigned long long* keys, void* v, unsigned char* c)
   {
     constexpr bool E = decltype (emit)::value;
@@ -2417,7 +2366,7 @@ int enumerate_leaves (b200tsdf* h, int nlevels, bool occupied, const char* what,
     const int nb = list_bricks (h, list);
     if (nb < 0) return nb;
     const int occ = occupied ? 1 : 0;
-    const unsigned bgrid = (unsigned) (((size_t) nb * 32 + 127) / 128), rgrid = (unsigned) ((h->root_n + 127) / 128);
+    const unsigned bgrid = (unsigned) (((size_t) nb * 32 + 127) / 128), rgrid = (unsigned) ((h->vol.root_n + 127) / 128);
     auto launch = [&] (auto emit, unsigned long long* total, unsigned long long* keys, void* rec, unsigned char*)
     {
       constexpr bool E = decltype (emit)::value;
@@ -2478,7 +2427,7 @@ int b200tsdf_debug_timing (b200tsdf_t* h, unsigned long long* out16)
   CK (cudaStreamSynchronize (h->stream));
   if (!h->d_dbg)
   {
-    CK (cudaMalloc (&h->d_dbg, 16 * 8)); CK (cudaMemset (h->d_dbg, 0, 16 * 8));
+    CK (h->d_dbg.grow (16)); CK (cudaMemset (h->d_dbg, 0, 16 * 8));
     h->p.dbg = h->d_dbg;                                   // armed from the next frame on (this handle only)
     drop_batch_graphs (h);
   }
@@ -2562,8 +2511,8 @@ int take_snapshot (b200tsdf* h, Snapshot& S)
   const int nb = list_bricks (h, d_list);
   if (nb < 0) return nb;
   std::vector<int> list (nb);
-  std::vector<uint64_t> dkeys (h->pool);
-  CK (cudaMemcpy (dkeys.data (), dp.keys, h->pool * sizeof (uint64_t), cudaMemcpyDeviceToHost));
+  std::vector<uint64_t> dkeys (h->vol.pool);
+  CK (cudaMemcpy (dkeys.data (), dp.keys, h->vol.pool * sizeof (uint64_t), cudaMemcpyDeviceToHost));
   if (nb) CK (cudaMemcpy (list.data (), d_list, (size_t) nb * sizeof (int), cudaMemcpyDeviceToHost));
   const size_t nn = (size_t) nb * BRICK_NODES;
   DevBuf<float2> g_nodes (s); DevBuf<uint32_t> g_split (s); DevBuf<uchar4> g_rgb (s); DevBuf<float> g_M (s); DevBuf<int> g_ns (s); DevBuf<float4> g_q (s);
@@ -2622,7 +2571,7 @@ int take_snapshot (b200tsdf* h, Snapshot& S)
       std::memcpy (&S.ns[(size_t) slot * BRICK_NODES], &c_ns[(size_t) i * BRICK_NODES], BRICK_NODES * sizeof (int));
     }
   }
-  size_t rn = h->root_n;
+  size_t rn = h->vol.root_n;
   S.root_dw.resize (rn); S.root_split.resize ((rn + 31) / 32);
   CK (cudaMemcpy (S.root_dw.data (), dp.root_dw, rn * sizeof (float2), cudaMemcpyDeviceToHost));
   CK (cudaMemcpy (S.root_split.data (), dp.root_split, S.root_split.size () * sizeof (uint32_t), cudaMemcpyDeviceToHost));
@@ -2907,7 +2856,7 @@ int b200tsdf_load (b200tsdf_t* h, const char* path)
   if (rc) { std::fclose (f); return rc; }
   const Params& p = h->p;
   VolLoader L; L.f = f; L.rgb = rgb; L.p = &p;
-  size_t rn = h->root_n;
+  size_t rn = h->vol.root_n;
   L.root_dw.assign (rn, make_float2 (-1.f, 0.f)); L.root_split.assign ((rn + 31) / 32, 0u);
   L.root_rgb.assign (rn, make_uchar4 (0, 0, 0, 0)); L.root_M.assign (rn, 0.f); L.root_ns.assign (rn, 0);
   L.node (0, 0, 0, 0);
@@ -3016,7 +2965,7 @@ int b200tsdf_import_shard (b200tsdf_t* h, const void* buf, size_t nbytes)
   {
     std::memcpy (&ridx[i], o, 4); o += 4; std::memcpy (&rdw[i], o, 8); o += 8; rsp[i] = *o++;
     std::memcpy (&rrgb[i], o, 4); o += 4; std::memcpy (&rM[i], o, 4); o += 4; std::memcpy (&rns[i], o, 4); o += 4;
-    if (ridx[i] < 0 || (size_t) ridx[i] >= h->root_n) return h->fail (B200TSDF_EINVAL, "corrupt shard buffer");
+    if (ridx[i] < 0 || (size_t) ridx[i] >= h->vol.root_n) return h->fail (B200TSDF_EINVAL, "corrupt shard buffer");
   }
   std::vector<uint64_t> keys (nb); std::vector<float2> nodes (nb * BRICK_NODES); std::vector<uint32_t> split (nb * BRICK_SPLIT_WORDS);
   std::vector<uchar4> rgb (color ? nb * BRICK_NODES : 0); std::vector<float> Mv (var ? nb * BRICK_NODES : 0); std::vector<int> nsv (var ? nb * BRICK_NODES : 0);

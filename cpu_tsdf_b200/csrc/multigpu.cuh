@@ -173,26 +173,24 @@ int b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows
   // two buffer sets, used alternately: set s is rewritten only after the batch that read it two calls ago has been fused
   const int s = h->rows_set;
   const size_t need_raw = hpack ? 0 : (size_t) HALF * per * width * stride, need_full = (size_t) HALF * frame16, need_pack = hpack ? (size_t) HALF * slice16 : 0;
-  if (need_raw > h->rows_raw_cap || need_full > h->rows_full_cap || need_pack > h->pack_cap)
+  auto fits = [&] (int k) { return need_raw <= h->d_rows_raw[k].cap && need_full <= h->d_rows_full[k].cap && need_pack <= h->h_pack[k].bytes; };
+  if (!fits (0) || !fits (1))
   {
     CK (cudaStreamSynchronize (h->stream)); CK (cudaStreamSynchronize (h->copy_stream)); CK (cudaStreamSynchronize (h->gather_stream));
     for (int k = 0; k < 2; ++k)
     {
-      cudaFree (h->d_rows_raw[k]); cudaFree (h->d_rows_full[k]); h->d_rows_raw[k] = h->d_rows_full[k] = nullptr;
-      h->h_pack[k].release ();
-      h->rows_raw_cap = h->rows_full_cap = h->pack_cap = 0;
-      if (need_raw) CK (cudaMalloc (&h->d_rows_raw[k], need_raw));
-      CK (cudaMalloc (&h->d_rows_full[k], need_full));
+      h->d_rows_raw[k].release (); h->d_rows_full[k].release (); h->h_pack[k].release ();
+      CK (h->d_rows_raw[k].grow (need_raw));
+      CK (h->d_rows_full[k].grow (need_full));
       if (need_pack && h->h_pack[k].alloc (need_pack))
       {
-        // no pinned staging to be had on this system: upload the points as they are from now on (the caps are 0: everything is re-sized)
+        // no pinned staging to be had on this system: upload the points as they are from now on (nothing fits: everything is re-sized)
         h->host_pack = 0;
         for (int j = 0; j < 2; ++j) h->h_pack[j].release ();
         return b200tsdf_integrate_batch_rows (h, n, rows, stride, xyz_off, rgba_off, width, height, poses_c2w);
       }
       h->rows_used[k] = false;
     }
-    h->rows_raw_cap = need_raw; h->rows_full_cap = need_full; h->pack_cap = need_pack;
   }
   if (hpack) ensure_pack_pool (h, nr);
   // three-stage pipeline over chunks of frames: the copy stream only uploads (the copy engine never waits for a kernel), the
@@ -332,7 +330,7 @@ int b200tsdf_gather_volume (b200tsdf_t* h, b200tsdf_t* full, int root)
   cudaStream_t s = h->stream;
   const Params& p = h->p;
   const bool color = p.rgb != nullptr;
-  const size_t rn = h->root_n, rsw = (rn + 31) / 32;
+  const size_t rn = h->vol.root_n, rsw = (rn + 31) / 32;
   // what this rank owns, packed on the device
   int* d_list = nullptr;
   const int nb = list_bricks (h, d_list);

@@ -72,7 +72,10 @@ const char* b200tsdf_last_error (const b200tsdf_t* h);
 int  b200tsdf_set_config (b200tsdf_t* h, const b200tsdf_config* cfg);
 int  b200tsdf_get_config (const b200tsdf_t* h, b200tsdf_config* cfg);
 
-/* TSDFVolumeOctree::reset (cpp:201-219) */
+/* TSDFVolumeOctree::reset (cpp:201-219).  B200TSDF_EINVAL for a configuration the engine refuses leaves the handle as it
+ * was, its volume included.  Any other failure (B200TSDF_ENOMEM when the device memory of the new volume cannot be had)
+ * leaves the handle without a volume: every call that needs one returns B200TSDF_ESTATE until a reset succeeds.
+ * b200tsdf_load resets the handle to the file's configuration and leaves it the same way when that reset fails. */
 int  b200tsdf_reset (b200tsdf_t* h);
 
 /* TSDFVolumeOctree::integrateCloud<PointT,NormalT> (include/cpu_tsdf/impl/
