@@ -825,6 +825,7 @@ struct b200tsdf
   DevBuf<uint32_t> d_fold; DevBuf<QNode> d_q1;
   uint32_t frame_seq = 0;        // FrameRec::seq of the last frame
   bool fold_prev = false;        // the last frame's route published fold marks (the next one on that route may be gated)
+  bool half_launched = false;    // a launch of a direct frame failed (part of it may be queued): calls refused until reset ()
   bool top_path = false; int sl = 0, nup = 0, super_static = 0;
   bool fast_path = false;
   // device copy of Params (the rare out-of-line paths read it through a pointer) and the ring of per-frame records
@@ -952,6 +953,7 @@ int check_device_err (b200tsdf* h)
 // by b200tsdf_sync / get_stats / mesh / save, instead of being served silently (ADVICE r1).
 int pending_device_err (b200tsdf* h)
 {
+  if (h->half_launched) return h->fail (B200TSDF_ESTATE, "an earlier frame was left half launched by a CUDA error; reset() the handle");
   const int e = *(volatile int*) h->h_err;
   if (!e) return 0;
   if (e & ERR_POOL_FULL) return h->fail (B200TSDF_ENOMEM, "brick pool exhausted in an earlier frame (raise pool_log2); the volume is incomplete");
@@ -1247,6 +1249,7 @@ int b200tsdf_reset (b200tsdf_t* h)
   h->count_set = 0;
   if (h->d_fold) CK (cudaMemsetAsync (h->d_fold, 0, h->d_fold.cap * sizeof (uint32_t), s));
   h->fold_prev = false;
+  h->half_launched = false;
   CK (cudaMemsetAsync (h->d_stats, 0, ST_TOTAL * sizeof (unsigned long long), s));
   h->kring_pending = 0; h->kring_head = 0;
   if (np.Rtop < np.C) k_insert_top_bricks<<<(unsigned) ((root_n + 127) / 128), 128, 0, s>>> (p);
@@ -1283,6 +1286,20 @@ static void fill_rec (b200tsdf* h, FrameRec& r, const unsigned char* d_pts, size
   h->fold_prev = pub;
   r.kt[0] = r.kt[1] = 0;
 }
+
+// The numbering fill_rec gives frames (seq, counter set, gate) becomes the handle's only once they are enqueued: a call that
+// fails before that puts it back on return, so that the next frame is numbered and gated as if the failed ones had never been
+// filled.  (A gated k_front waits for `opened == seq - 1`, which a frame that was numbered but never launched would not publish.)
+// Every argument is checked before the first fill_rec, so only a CUDA error can still fail here.  A launch that fails inside
+// launch_frame outside a graph may leave part of that frame on the stream: integrate_on_device then latches half_launched, so
+// that every later call that would queue work on the handle returns B200TSDF_ESTATE until reset (), which starts the numbering
+// afresh (counter set 0, no gate, fold marks cleared).
+struct FrameNumbering
+{
+  b200tsdf* h; uint32_t seq; int cset; bool fold_prev; bool enqueued = false;
+  explicit FrameNumbering (b200tsdf* h_) : h (h_), seq (h_->frame_seq), cset (h_->count_set), fold_prev (h_->fold_prev) {}
+  ~FrameNumbering () { if (!enqueued) { h->frame_seq = seq; h->count_set = cset; h->fold_prev = fold_prev; } }
+};
 
 // the launches of one frame; every kernel reads the frame from *d_rec, so the launches can be captured and replayed.
 // with_events: bracket the dominant kernel with an event pair of the ring (never inside a capture)
@@ -1391,10 +1408,12 @@ static int integrate_on_device (b200tsdf* h, const unsigned char* d_pts, size_t 
   int slot = 0;
   { int rc = ring_slot (h, slot); if (rc) return rc; }
   FrameRec& rec = h->h_ring[slot];
+  FrameNumbering num (h);
   fill_rec (h, rec, d_pts, stride, xyz_off, rgba_off, W, H, pose);
   if (h->time_frames) CK (cudaEventRecord (h->ev_t0, s));
   CK (cudaMemcpyAsync (h->d_ring + slot, &rec, sizeof (FrameRec), cudaMemcpyHostToDevice, s));
-  { int rc = launch_frame (h, s, h->d_ring + slot, h->time_frames); if (rc) return rc; }
+  { int rc = launch_frame (h, s, h->d_ring + slot, h->time_frames); if (rc) { h->half_launched = true; return rc; } }
+  num.enqueued = true;
   if (h->time_frames) CK (cudaEventRecord (h->ev_t1, s));
   note_device_err (h, s);
   { int rc = ring_advance (h, slot, s); if (rc) return rc; }
@@ -1433,6 +1452,7 @@ int b200tsdf_integrate_device (b200tsdf_t* h, const void* d_points, size_t strid
 // path (multigpu.cuh) uploads the records on its copy stream AHEAD of the frames themselves — a record upload issued on
 // the compute stream would queue behind every frame copy already submitted to the one host-to-device copy engine.
 // ob / orecs: the organise block of an unorganised batch, which travels in the same copy behind the frame records
+// The caller has checked every argument (d_points[i] are not null) and holds a FrameNumbering until batch_launch has returned.
 static int batch_records (b200tsdf* h, int m, const void* const* d_points, size_t stride, int xyz_off, int rgba_off, int width, int height,
                           const double* poses_c2w, cudaStream_t rec_stream, const OrgBatch* ob = nullptr, const OrgRec* orecs = nullptr)
 {
@@ -1440,10 +1460,7 @@ static int batch_records (b200tsdf* h, int m, const void* const* d_points, size_
   if (h->bring_used[sg]) CK (cudaEventSynchronize (h->ev_bring[sg]));    // the copy that last read this staging segment has run
   FrameRec* recs = h->h_bring + (size_t) sg * BRING_SPAN;
   for (int i = 0; i < m; ++i)
-  {
-    if (!d_points[i]) return h->fail (B200TSDF_EINVAL, "null cloud in batch");
     fill_rec (h, recs[i], (const unsigned char*) d_points[i], stride, xyz_off, rgba_off, width, height, poses_c2w + 16 * (size_t) i);
-  }
   size_t bytes = (size_t) m * sizeof (FrameRec);
   if (ob)
   {
@@ -1527,14 +1544,18 @@ int b200tsdf_integrate_batch_device (b200tsdf_t* h, int n, const void* const* d_
   if (!h || n < 0 || (n && (!d_points || !poses_c2w))) return B200TSDF_EINVAL;
   if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "integrateCloud before reset()");
   if (int rc = check_cloud_layout (h, stride, xyz_off, rgba_off, width, height)) return rc;
+  // every pointer of every record half, before any of them is numbered or fused: a refused batch enqueues nothing
+  for (int i = 0; i < n; ++i) if (!d_points[i]) return h->fail (B200TSDF_EINVAL, "null cloud in batch");
   cudaSetDevice (h->device);
   if (int rc = pending_device_err (h)) return rc;
   constexpr int HALF = FRAME_RING / 2;
   for (int done = 0; done < n;)
   {
     const int m = std::min (HALF, n - done);
+    FrameNumbering num (h);
     if (int rc = batch_records (h, m, d_points + done, stride, xyz_off, rgba_off, width, height, poses_c2w + 16 * (size_t) done, h->stream)) return rc;
     if (int rc = batch_launch (h, m)) return rc;
+    num.enqueued = true;
     done += m;
   }
   CK (cudaGetLastError ());
@@ -1718,8 +1739,10 @@ int unorganized_batches (b200tsdf* h, int n, const void* const* d_points, const 
       recs[i] = org_rec (d_points[k], counts[k], first, opts->world_to_camera ? opts->world_to_camera + 16 * (size_t) k : nullptr);
       first += counts[k];
     }
+    FrameNumbering num (h);
     if (int rc = batch_records (h, m, imgs, 16, 0, 12, h->cfg.image_width, h->cfg.image_height, poses_c2w + 16 * (size_t) done, h->stream, &ob, recs)) return rc;
     if (int rc = batch_launch (h, m, true)) return rc;
+    num.enqueued = true;
     done += m;
   }
   CK (cudaGetLastError ());

@@ -159,6 +159,8 @@ int b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows
   const int per = (height + nr - 1) / nr;                       // rows per rank (the last rank's slice may be short)
   const int row0 = std::min (height, rk * per), row1 = std::min (height, (rk + 1) * per);
   const size_t slice_raw = (size_t) (row1 - row0) * width * stride;
+  // every argument is checked before anything is synchronised, re-sized, numbered or enqueued: a refused batch enqueues nothing
+  for (int i = 0; i < n; ++i) if (!rows[i] && slice_raw) return h->fail (B200TSDF_EINVAL, "null row slice in batch");
   const size_t slice16 = (size_t) per * width * 16, frame16 = slice16 * nr;
   // host packing (host_pack.h): the caller's rows are packed to 16-byte pixels by host threads into pinned staging and only
   // those cross PCIe; without it the points are uploaded as they are (and packed on the device when there is a gather)
@@ -201,7 +203,6 @@ int b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows
   if (h->rows_used[s]) { CK (cudaStreamWaitEvent (cs, h->ev_rows_done[s], 0)); CK (cudaStreamWaitEvent (gs, h->ev_rows_done[s], 0)); }
   const int npts = (row1 - row0) * width;
   const int out_rgba = (h->p.color && rgba_off >= 0) ? 12 : -1;
-  for (int i = 0; i < n; ++i) if (!rows[i] && slice_raw) return h->fail (B200TSDF_EINVAL, "null row slice in batch");
   int cbeg[HALF + 1];
   const int nchunks = b2host::stage_schedule (n, ROWS_CHUNK, cbeg);
   static const bool trace = std::getenv ("B200TSDF_TRACE_ROWS") != nullptr;
@@ -252,6 +253,7 @@ int b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows
         if (!h->pack_pool->help ()) std::this_thread::yield ();
     if (trace) { const double t = now (); t_pack += t - t0; t0 = t; }
     // the chunk's frame records travel on the copy stream ahead of its frames
+    FrameNumbering num (h);
     if (int rc = batch_records (h, m, ptrs, f_stride, f_xyz, f_rgba, width, height, poses_c2w + 16 * (size_t) c0, cs)) return rc;
     if (hpack)
     {
@@ -296,6 +298,7 @@ int b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows
     }
     CK (cudaStreamWaitEvent (h->stream, ready, 0));
     if (int rc = batch_launch (h, m)) return rc;
+    num.enqueued = true;
     if (trace) t_enq += now () - t0;
   }
   CK (cudaEventRecord (h->ev_rows_done[s], h->stream));

@@ -98,13 +98,16 @@ int  b200tsdf_integrate_device (b200tsdf_t* h, const void* d_points, size_t stri
  * per batch size, replayed afterwards), so the host issues ~3 driver calls per batch instead of ~6 per frame.
  * d_points: n device pointers (same layout for all); poses_c2w: n row-major 4x4 matrices back to back.  Asynchronous
  * like b200tsdf_integrate_device.  Every configuration takes this path, those fused by the general depth-first kernel
- * (track_variance, RGBNormalized payload) included. */
+ * (track_variance, RGBNormalized payload) included.  Every argument of every frame is checked before the first frame is
+ * fused: a refused call (B200TSDF_EINVAL, e.g. a NULL pointer anywhere in d_points) enqueues nothing and leaves the handle
+ * as it was. */
 int  b200tsdf_integrate_batch_device (b200tsdf_t* h, int n, const void* const* d_points, size_t stride, int xyz_off, int rgba_off,
                                       int width, int height, const double* poses_c2w);
 /* streaming variant of b200tsdf_integrate for producers that keep their (pinned) frame buffers alive:
  * returns as soon as the copy and the kernels are enqueued.  `points` must stay valid and unmodified
- * until b200tsdf_sync() or until two further frames have been submitted on this handle (the call that submits
- * frame i+2 waits for the upload of frame i before it returns); when the upload is packed on the host (see
+ * until b200tsdf_sync() or until two further frames have been submitted on this handle by b200tsdf_integrate or
+ * b200tsdf_integrate_async (the call that submits frame i+2 of these two waits for the upload of frame i before it returns;
+ * frames of the other entry points do not count); when the upload is packed on the host (see
  * b200tsdf_integrate) the buffer is already free on return.
  * Error reporting of the asynchronous entry points (integrate_device / _batch_device / _async, and integrate itself, which
  * waits for its upload only): a device-side failure of frame i (brick pool exhausted, work queue overflow) is reported by
@@ -143,7 +146,8 @@ int  b200tsdf_integrate_unorganized (b200tsdf_t* h, const void* points, size_t n
  * opts->world_to_camera: NULL or n row-major 4x4 matrices back to back; cloud_units and zero_nans apply to every cloud.
  * poses_c2w: n row-major 4x4 matrices back to back.  Every 32 frames are organised and fused by one CUDA-graph launch
  * (captured once per batch size, replayed afterwards).  Asynchronous on the handle's stream; errors as for
- * b200tsdf_integrate_device.  B200TSDF_EINVAL for a bad argument, B200TSDF_ESTATE before reset(), B200TSDF_ENOMEM when the
+ * b200tsdf_integrate_device.  B200TSDF_EINVAL for a bad argument of any frame (a refused call enqueues nothing and leaves the
+ * handle as it was), B200TSDF_ESTATE before reset(), B200TSDF_ENOMEM when the
  * organised images (32 * image_width * image_height * 24 bytes, allocated at the first unorganised integrate and freed by
  * reset()) do not fit. */
 int  b200tsdf_integrate_unorganized_batch_device (b200tsdf_t* h, int n, const void* const* d_points, const size_t* counts,
@@ -270,7 +274,10 @@ int  b200tsdf_row_slice (const b200tsdf_t* h, int height, int* row0, int* row1);
  * GPU's PCIe link, packed to 16-byte pixels and all-gathered over NVLink into the full frame on every rank (collective: all
  * ranks call with the same n), then the batch is fused like b200tsdf_integrate_batch_device.  Without a communicator the
  * slice is the whole frame and nothing is exchanged.  With a single rank the slice is packed on the host first (see
- * b200tsdf_integrate) and rows[i] are free on return; otherwise they must stay valid until b200tsdf_sync or two further calls. */
+ * b200tsdf_integrate) and rows[i] are free on return; otherwise they must stay valid until b200tsdf_sync or two further calls
+ * of this entry point.
+ * B200TSDF_EINVAL for n > 32, a NULL row slice or a bad layout: a refused call enqueues nothing and leaves the handle as it
+ * was.  n == 0 returns B200TSDF_OK and does nothing. */
 int  b200tsdf_integrate_batch_rows (b200tsdf_t* h, int n, const void* const* rows, size_t stride, int xyz_off, int rgba_off,
                                     int width, int height, const double* poses_c2w);
 /* Collective: every rank's shard goes device to device (NCCL send/recv over NVLink, no host staging) to rank `root`, which
