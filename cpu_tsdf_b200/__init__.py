@@ -74,7 +74,7 @@ EXPORTS = [
     "b200tsdf_integrate_device", "b200tsdf_integrate_batch_device", "b200tsdf_integrate_async",
     "b200tsdf_comm_unique_id", "b200tsdf_comm_init", "b200tsdf_row_slice", "b200tsdf_integrate_batch_rows", "b200tsdf_gather_volume", "b200tsdf_sync", "b200tsdf_organize", "b200tsdf_integrate_unorganized", "b200tsdf_integrate_unorganized_batch_device", "b200tsdf_query", "b200tsdf_interpolate", "b200tsdf_render", "b200tsdf_mesh",
     "b200tsdf_query_device", "b200tsdf_interpolate_device", "b200tsdf_render_batch_device",
-    "b200tsdf_free", "b200tsdf_save", "b200tsdf_load", "b200tsdf_export_shard", "b200tsdf_import_shard", "b200tsdf_voxel_center", "b200tsdf_voxel_index",
+    "b200tsdf_free", "b200tsdf_save", "b200tsdf_load", "b200tsdf_save_device", "b200tsdf_load_device", "b200tsdf_load_path", "b200tsdf_export_shard", "b200tsdf_import_shard", "b200tsdf_voxel_center", "b200tsdf_voxel_index",
     "b200tsdf_voxel_centers", "b200tsdf_occupied_voxel_indices", "b200tsdf_is_empty",
     "b200tsdf_get_stats", "b200tsdf_download_nodes", "b200tsdf_download_color_payload", "b200tsdf_frustum_cull",
     "b200tsdf_profile_begin", "b200tsdf_profile_end",
@@ -149,6 +149,9 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_mesh_cleanup_device.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, C.c_float, C.c_int, vp, vp, szp, szp]
     lib.b200tsdf_save.argtypes = [vp, C.c_char_p]
     lib.b200tsdf_load.argtypes = [vp, C.c_char_p]
+    lib.b200tsdf_save_device.argtypes = [vp, vp, C.c_size_t, szp]
+    lib.b200tsdf_load_device.argtypes = [vp, vp, C.c_size_t]
+    lib.b200tsdf_load_path.argtypes = [vp, C.POINTER(C.c_int32)]
     lib.b200tsdf_export_shard.argtypes = [vp, vp, C.c_size_t, C.POINTER(C.c_size_t)]
     lib.b200tsdf_import_shard.argtypes = [vp, vp, C.c_size_t]
     lib.b200tsdf_voxel_center.argtypes = [vp, C.c_int64, C.c_int64, C.c_int64, vp]
@@ -510,6 +513,26 @@ class TSDFVolumeOctree:
         """cpp:248-275 — adopts the file's configuration and rebuilds the volume on the device."""
         self._check(self._lib.b200tsdf_load(self._h, filename.encode()))
         self._check(self._lib.b200tsdf_get_config(self._h, C.byref(self._cfg)))
+
+    def saveDevice(self, d_buf: int | None = None, capacity: int = 0) -> int:
+        """save() into device memory of the volume's device (an integer device pointer, e.g. a torch tensor's data_ptr()):
+        the same bytes as the file.  Returns the image's size; d_buf=None returns it without writing, and a capacity below
+        it raises with nothing written."""
+        n = C.c_size_t()
+        self._check(self._lib.b200tsdf_save_device(self._h, C.c_void_p(d_buf) if d_buf else None, int(capacity), C.byref(n)))
+        return n.value
+
+    def loadDevice(self, d_buf: int, nbytes: int):
+        """load() of a .vol image of nbytes bytes in device memory of the volume's device (e.g. one saveDevice wrote)."""
+        self._check(self._lib.b200tsdf_load_device(self._h, C.c_void_p(d_buf) if d_buf else None, int(nbytes)))
+        self._check(self._lib.b200tsdf_get_config(self._h, C.byref(self._cfg)))
+
+    def loadPath(self) -> str:
+        """"device" when the last load() / loadDevice() placed the file's body with the device parser, "host" when the host
+        loader did or the volume comes from reset()."""
+        out = C.c_int32()
+        self._check(self._lib.b200tsdf_load_path(self._h, C.byref(out)))
+        return "device" if out.value else "host"
 
     def export_shard(self) -> np.ndarray:
         """Everything this (sharded) handle owns, as a byte buffer that any transport can ship (DESIGN.md §5)."""

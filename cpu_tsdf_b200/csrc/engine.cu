@@ -12,6 +12,7 @@
 #include "organize.cuh"
 #include "mesh_sort.h"
 #include "host_pack.h"
+#include "vol_io.cuh"
 
 #include <cuda_runtime.h>
 #include <sys/mman.h>
@@ -726,6 +727,140 @@ __global__ void k_leaves_level (Params gp, int level, unsigned long long count, 
   leaf_record (p, level, x, y, z, false, rec + 3 * i);
 }
 
+// ---- .vol save on the device (DESIGN.md §3e): every node of the walk as a VolNode with its pre-order key, sorted, then
+// formatted into byte-packed records ----
+
+// the root-array entries, and the geometry-only levels above them: the ancestor at level l < Rtop is emitted by the entry
+// whose coordinates are its child-0 chain
+template <bool EMIT>
+__global__ void k_vol_roots (Params gp, unsigned long long* __restrict__ total, unsigned long long* __restrict__ okeys, VolNode* __restrict__ out)
+{
+  B2_STAGE_PARAMS (gp)
+  const int n = 1 << p.Rtop;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int z = i % n, y = (i / n) % n, x = i / (n * n);
+  int cnt = 0;
+  if (i < n * n * n)                                           // (the block size is a multiple of 32: every lane reaches warp_reserve)
+  {
+    cnt = 1;
+    for (int l = p.Rtop - 1; l >= 0; --l)
+    {
+      const int m = (1 << (p.Rtop - l)) - 1;
+      if ((x & m) || (y & m) || (z & m)) break;
+      ++cnt;
+    }
+  }
+  unsigned long long o;
+  if (!warp_reserve (total, cnt, o)) return;
+  if (!EMIT || !cnt) return;
+  const NodePos nd = make_root (p, x, y, z);
+  okeys[o] = vol_key (p, p.Rtop, x, y, z);
+  out[o] = vol_node (okeys[o], -1, nd.idx, vol_has_children (p, nd));
+  for (int c = 1; c < cnt; ++c)
+  {
+    const int l = p.Rtop - c;
+    okeys[o + c] = vol_key (p, l, x >> c, y >> c, z >> c);
+    out[o + c] = vol_node (okeys[o + c], VOL_SLOT_GEOM, 0, true);
+  }
+}
+
+// every node of every claimed brick whose root has children: one warp per brick, through brick_node as the mesh and the leaf
+// lists walk it
+template <bool EMIT>
+__global__ void k_vol_bricks (Params gp, const int* __restrict__ list, int nbricks, unsigned long long* __restrict__ total,
+                              unsigned long long* __restrict__ okeys, VolNode* __restrict__ out)
+{
+  B2_STAGE_PARAMS (gp)
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= nbricks) return;
+  const int slot = list[warp];
+  int t, bx, by, bz;
+  brick_key_decode (p.keys[slot], t, bx, by, bz);
+  if (!brick_root_is_split (p, t, bx, by, bz)) return;
+  const int R = tier_root_level (p, t);
+  const uint32_t* sw = p.split + (size_t) slot * BRICK_SPLIT_WORDS;
+  for (int base = 0; base < BRICK_NODES; base += 32)
+  {
+    const int i = base + lane;
+    BrickNode b{};
+    bool sel = false;
+    if (i < BRICK_NODES)
+    {
+      b = brick_node (p, sw, R, bx, by, bz, true, i);
+      sel = b.exists;
+    }
+    unsigned long long o;
+    if (!warp_reserve (total, sel ? 1 : 0, o)) continue;
+    if (EMIT && sel)
+    {
+      NodePos n; n.level = b.level; n.x = b.x; n.y = b.y; n.z = b.z; n.slot = slot; n.idx = i;
+      const bool children = b.split && children_slot (p, n, false) >= 0;
+      okeys[o] = vol_key (p, b.level, b.x, b.y, b.z);
+      out[o] = vol_node (okeys[o], slot, i, children);
+    }
+  }
+}
+
+// the sorted nodes [first, first + n) as byte-packed records at out: each thread formats one record into shared memory, then
+// the block copies its records out in one coalesced run
+constexpr int VOL_FORMAT_THREADS = 256;
+__global__ void __launch_bounds__ (VOL_FORMAT_THREADS) k_vol_format (Params gp, const VolNode* __restrict__ nodes, size_t first, size_t n,
+                                                                      int rbytes, unsigned char* __restrict__ out)
+{
+  B2_STAGE_PARAMS (gp)
+  __shared__ unsigned char buf[VOL_FORMAT_THREADS * 44];
+  const size_t b0 = (size_t) blockIdx.x * VOL_FORMAT_THREADS;
+  const size_t i = b0 + threadIdx.x;
+  if (i < n) vol_format (p, nodes[first + i], buf + threadIdx.x * rbytes);
+  __syncthreads ();
+  const size_t m = min ((size_t) VOL_FORMAT_THREADS, n - b0) * (size_t) rbytes;
+  unsigned char* o = out + b0 * rbytes;
+  for (size_t k = threadIdx.x; k < m; k += VOL_FORMAT_THREADS) o[k] = buf[k];
+}
+
+// ---- .vol load on the device: one record per thread ----
+
+// nchild - 1 of each record: the open-slot count after record i is 1 + the inclusive sum up to i
+__global__ void k_vol_slots (const unsigned char* __restrict__ body, size_t nrec, int rbytes, long long* __restrict__ delta)
+{
+  const size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nrec) return;
+  unsigned long long nchild;
+  vol_get (body + i * rbytes + rbytes - 8, &nchild, 8);
+  delta[i] = nchild == 8 ? 7 : -1;
+}
+
+// res[0] = the first record after which no slot is open (min over the records that close the tree)
+__global__ void k_vol_end (const long long* __restrict__ incl, size_t nrec, unsigned long long* __restrict__ res)
+{
+  const size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nrec && incl[i] == -1) atomicMin (res, (unsigned long long) i);
+}
+
+// every check of records [0, n): res[1] = records that fail, res[2] = stored {d, w} outside the fast route's domain
+__global__ void k_vol_check (Params gp, const unsigned char* __restrict__ body, size_t n, int rbytes, int rgb, unsigned long long* __restrict__ res)
+{
+  B2_STAGE_PARAMS (gp)
+  const size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+  bool bad = false, out = false;
+  if (i < n) bad = !vol_check_record (p, body, i, n, rbytes, rgb != 0, out);
+  const unsigned mb = __ballot_sync (0xffffffffu, bad), mo = __ballot_sync (0xffffffffu, out);
+  if ((threadIdx.x & 31) == 0)
+  {
+    if (mb) atomicAdd (res + 1, (unsigned long long) __popc (mb));
+    if (mo) atomicAdd (res + 2, (unsigned long long) __popc (mo));
+  }
+}
+
+// records [0, n), all checked, into the freshly reset volume: vol_place as the host loader places them
+__global__ void k_vol_place (Params gp, const unsigned char* __restrict__ body, size_t n, int rbytes, int rgb)
+{
+  B2_STAGE_PARAMS (gp)
+  const size_t i = (size_t) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  vol_store (p, vol_parse (p, body + i * rbytes, rgb != 0));
+}
+
 } // namespace
 
 // ---------------------------------------------------------------------------------------------
@@ -812,6 +947,7 @@ struct b200tsdf
   bool timed = false;
   bool time_frames = false;      // set between profile_begin / profile_end: per-frame event records (ev_t0/ev_t1 and the ring around the dominant kernel)
   bool is_empty = true;          // TSDFVolumeOctree::is_empty_ (cpp:205, hpp:101)
+  bool loaded_on_device = false; // the last load placed its body with the device parser (b200tsdf_load_path)
   // fast-path work queues (levels C .. L-3), and the lists of block roots, BL_CLASSES lists of blist_cap () entries
   Queues Q{}; int q_levels = 0; DevBuf<QNode> q_mem;
   DevBuf<int> d_blist;
@@ -1259,6 +1395,7 @@ int b200tsdf_reset (b200tsdf_t* h)
   h->frame_no = 0;
   h->timed = false;
   h->is_empty = true;
+  h->loaded_on_device = false;
   h->has_volume = true;
   return check_device_err (h);
 }
@@ -2744,18 +2881,32 @@ int64_t b200tsdf_download_color_payload (b200tsdf_t* h, float* out4)
   return (int64_t) recs.size ();
 }
 
-// save (tsdf_volume_octree.cpp:222-245; Octree::serialize octree.cpp:645-657; serializeASCII
-// eigen_extensions.h:249-257)
-int b200tsdf_save (b200tsdf_t* h, const char* path)
+} // extern "C"
+
+// ---- .vol save and load (DESIGN.md §3e) ------------------------------------------------------------------------------------
+namespace {
+
+constexpr int VOL_HOST_IO = 4;                      // debug_flags bit 2 (of the configuration set last): .vol through the host
+                                                    // writer and the host loader
+constexpr size_t VOL_CHUNK = (size_t) 1 << 19;      // records per pinned staging buffer of the file writer
+constexpr size_t VOL_LOAD_CHUNK = (size_t) 1 << 25; // bytes per pinned staging buffer of the file loader
+constexpr size_t VOL_HEAD_PROBE = (size_t) 1 << 16; // bytes of a device image copied to the host for its header
+
+struct File
 {
-  if (!h || !path) return B200TSDF_EINVAL;
-  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "save before reset()");
-  Snapshot S;
-  int rc = take_snapshot (h, S);
-  if (rc) return rc;
+  std::FILE* f = nullptr;
+  File (const File&) = delete;
+  File& operator= (const File&) = delete;
+  explicit File (std::FILE* x) : f (x) {}
+  ~File () { if (f) std::fclose (f); }
+  operator std::FILE* () const { return f; }
+};
+
+// the text header (tsdf_volume_octree.cpp:222-245; serializeASCII eigen_extensions.h:249-257) and the octree header
+// (Octree::serialize octree.cpp:645-657: the resolution as three size_t, the size as three float) in front of the body
+std::string vol_header (const b200tsdf* h)
+{
   const b200tsdf_config& c = h->cfg;
-  std::FILE* f = std::fopen (path, "wb");
-  if (!f) return h->fail (B200TSDF_EIO, std::string ("cannot open ") + path);
   std::string hd = "# TSDFVolumeOctree Meta Information\n";
   hd += std::to_string (c.xres) + " " + std::to_string (c.yres) + " " + std::to_string (c.zres) + "\n";
   hd += fmt16 (c.xsize) + " " + fmt16 (c.ysize) + " " + fmt16 (c.zsize) + "\n";
@@ -2773,11 +2924,23 @@ int b200tsdf_save (b200tsdf_t* h, const char* path)
     for (int k = 0; k < 4; ++k) { if (k) hd += " "; hd += std::string (width - cell[r * 4 + k].size (), ' ') + cell[r * 4 + k]; }
     hd += "\n";
   }
-  hd += std::string (S.p.color_norm ? "RGBNormalized" : (S.p.color ? "RGB" : "NOCOLOR")) + "\n#OCTREEBINARY\n";
+  hd += std::string (h->p.color_norm ? "RGBNormalized" : (h->p.color ? "RGB" : "NOCOLOR")) + "\n#OCTREEBINARY\n";
+  const size_t res[3] = { (size_t) c.xres, (size_t) c.yres, (size_t) c.zres };
+  hd.append ((const char*) res, sizeof (res));
+  hd.append ((const char*) &c.xsize, 4); hd.append ((const char*) &c.ysize, 4); hd.append ((const char*) &c.zsize, 4);
+  return hd;
+}
+
+// the host writer: a host snapshot walked recursively (write_vol_node)
+int save_host (b200tsdf* h, const char* path)
+{
+  Snapshot S;
+  int rc = take_snapshot (h, S);
+  if (rc) return rc;
+  std::FILE* f = std::fopen (path, "wb");
+  if (!f) return h->fail (B200TSDF_EIO, std::string ("cannot open ") + path);
+  const std::string hd = vol_header (h);
   std::fwrite (hd.data (), 1, hd.size (), f);
-  size_t res[3] = { (size_t) c.xres, (size_t) c.yres, (size_t) c.zres };
-  std::fwrite (res, sizeof (size_t), 3, f);
-  std::fwrite (&c.xsize, 4, 1, f); std::fwrite (&c.ysize, 4, 1, f); std::fwrite (&c.zsize, 4, 1, f);
   NodePos root;
   root.level = 0; root.x = root.y = root.z = 0; root.cx = root.cy = root.cz = 0.f; root.size = S.p.size; root.slot = -1; root.idx = 0;
   write_vol_node (S.p, f, root, S.p.Rtop == 0);
@@ -2786,13 +2949,126 @@ int b200tsdf_save (b200tsdf_t* h, const char* path)
   return bad ? h->fail (B200TSDF_EIO, "write failed") : B200TSDF_OK;
 }
 
+// Every node of the volume as a VolNode, sorted into the file's order in `nodes` (`count` of them), after the work queued
+// on the handle.  admit (count, go) sees the count first: it may refuse (its error is returned) or leave go false to stop
+// there.
+template <typename Admit>
+int vol_walk (b200tsdf* h, DevBuf<VolNode>& nodes, unsigned long long& count, const Admit& admit)
+{
+  int* d_list = nullptr;
+  const int nb = list_bricks (h, d_list);
+  if (nb < 0) return nb;
+  const Params& p = h->p;
+  cudaStream_t s = h->stream;
+  const unsigned nroot = 1u << (3 * p.Rtop);
+  auto launch = [&] (auto emit, unsigned long long* total, unsigned long long* k, uint32_t* v, unsigned char*)
+  {
+    constexpr bool E = decltype (emit)::value;
+    k_vol_roots<E><<<(nroot + 127) / 128, 128, 0, s>>> (p, total, k, (VolNode*) v);
+    if (nb) k_vol_bricks<E><<<(unsigned) ((nb + 3) / 4), 128, 0, s>>> (p, d_list, nb, total, k, (VolNode*) v);
+  };
+  auto dest = [&] (unsigned long long n, void*& v_out, unsigned char*&)
+  {
+    bool go = false;
+    if (int rc = admit (n, go)) return rc;
+    if (!go || !n) return (int) B200TSDF_OK;
+    if (nodes.alloc ((size_t) n)) return alloc_failed (h, "vol records");
+    v_out = nodes.p;
+    return (int) B200TSDF_OK;
+  };
+  static_assert (sizeof (VolNode) == 16, "a VolNode is four sort words");
+  return sorted_records (h, "vol records", 4, 3 * p.L + VOL_KEY_LEVEL_BITS, launch, dest, count);
+}
+
+void vol_format_launch (b200tsdf* h, const VolNode* nodes, size_t first, size_t n, unsigned char* out)
+{
+  const int rb = vol_record_bytes (h->p.color != 0, h->p.color_norm != 0);
+  if (n) k_vol_format<<<(unsigned) ((n + VOL_FORMAT_THREADS - 1) / VOL_FORMAT_THREADS), VOL_FORMAT_THREADS, 0, h->stream>>> (h->p, nodes, first, n, rb, out);
+}
+
+// the device writer into a file: the sorted nodes are formatted a chunk at a time, and the D2H copy of each chunk into one
+// of two pinned buffers overlaps the fwrite of the one before
+int save_device_file (b200tsdf* h, const char* path)
+{
+  if (int rc = b200tsdf_sync (h)) return rc;
+  cudaStream_t s = h->stream;
+  DevBuf<VolNode> nodes (s);
+  unsigned long long count = 0;
+  if (int rc = vol_walk (h, nodes, count, [] (unsigned long long, bool& go) { go = true; return (int) B200TSDF_OK; })) return rc;
+  const size_t rb = (size_t) vol_record_bytes (h->p.color != 0, h->p.color_norm != 0);
+  const size_t chunk = std::max<size_t> (1, std::min<size_t> (VOL_CHUNK, (size_t) count));
+  DevBuf<unsigned char> d_chunk (s);
+  Pinned<unsigned char> pin[2];
+  Event ev[2];
+  if (d_chunk.alloc (chunk * rb)) return alloc_failed (h, "vol staging");
+  for (int k = 0; k < 2; ++k)
+  {
+    if (pin[k].alloc (chunk * rb) != cudaSuccess) { cudaGetLastError (); return h->fail (B200TSDF_ENOMEM, "pinned host allocation failed"); }
+    CK (cudaEventCreateWithFlags (&ev[k].x, cudaEventDisableTiming));
+  }
+  File f (std::fopen (path, "wb"));
+  if (!f) return h->fail (B200TSDF_EIO, std::string ("cannot open ") + path);
+  const std::string hd = vol_header (h);
+  std::fwrite (hd.data (), 1, hd.size (), f);
+  int last = -1; size_t pending = 0;
+  for (size_t first = 0, k = 0; first < count; first += chunk, ++k)
+  {
+    const size_t n = std::min<size_t> (chunk, (size_t) count - first);
+    const int b = (int) (k & 1);
+    vol_format_launch (h, nodes, first, n, d_chunk);
+    CK (cudaMemcpyAsync (pin[b], d_chunk, n * rb, cudaMemcpyDeviceToHost, s));
+    CK (cudaEventRecord (ev[b], s));
+    if (last >= 0) { CK (cudaEventSynchronize (ev[last])); std::fwrite (pin[last], 1, pending, f); }
+    last = b; pending = n * rb;
+  }
+  if (last >= 0) { CK (cudaEventSynchronize (ev[last])); std::fwrite (pin[last], 1, pending, f); }
+  CK (cudaGetLastError ());
+  const bool bad = std::ferror (f) != 0;
+  const bool closed = std::fclose (f.f) == 0;
+  f.f = nullptr;
+  return (bad || !closed) ? h->fail (B200TSDF_EIO, "write failed") : B200TSDF_OK;
+}
 
 // ---- load (tsdf_volume_octree.cpp:248-275; Octree::deserialize octree.cpp:659-678; OctreeNode::deserialize :306-325) ----
-namespace {
+
+// the text and octree headers from f into c (the handle's pending configuration with the file's values), rgb and is_empty;
+// `name` prefixes the messages.  f is left at the first body byte.
+int vol_read_header (b200tsdf* h, std::FILE* f, const std::string& name, b200tsdf_config& c, bool& rgb, int& is_empty)
+{
+  c = h->cfg_pending;
+  char line[1024];
+  auto fail = [&] (const std::string& m) { return h->fail (B200TSDF_EIO, name + ": " + m); };
+  if (!std::fgets (line, sizeof (line), f)) return fail ("empty file");
+  int wd = 0, wv = 0;
+  is_empty = 0;
+  double gt[16];
+  int nread = std::fscanf (f, "%d %d %d %f %f %f %f %f %f %f %f %f %f %f %lf %lf %lf %lf %d %d %d %d %d",
+                           &c.xres, &c.yres, &c.zres, &c.xsize, &c.ysize, &c.zsize, &c.max_dist_pos, &c.max_dist_neg, &c.max_weight,
+                           &c.min_sensor_dist, &c.max_sensor_dist, &c.max_cell_x, &c.max_cell_y, &c.max_cell_z,
+                           &c.fx, &c.fy, &c.cx, &c.cy, &c.image_width, &c.image_height, &is_empty, &wd, &wv);
+  if (nread != 23) return fail ("bad header");
+  // the reference has no setter for these two: only a .vol written with them set turns the alternative weightings on (hpp:200-204)
+  if (wd || wv) return fail ("weight_by_depth_ / weight_by_variance_ volumes are not supported (the fusion here uses w_new = 1)");
+  char pct[8]; int rr = 0, cc = 0;
+  if (std::fscanf (f, " %1s %d %d", pct, &rr, &cc) != 3 || pct[0] != '%' || rr != 4 || cc != 4) return fail ("bad transform header");
+  for (int i = 0; i < 16; ++i) if (std::fscanf (f, "%lf", &gt[i]) != 1) return fail ("bad transform");
+  char type[64];
+  if (std::fscanf (f, "%63s", type) != 1) return fail ("missing node type");
+  rgb = std::string (type) == "RGB";
+  if (!rgb && std::string (type) != "NOCOLOR") return fail (std::string ("unsupported node type ") + type);
+  do { if (!std::fgets (line, sizeof (line), f)) return fail ("missing #OCTREEBINARY"); } while (!(line[0] == '#' && line[1] == 'O'));
+  size_t res3[3]; float size3[3];
+  if (std::fread (res3, sizeof (size_t), 3, f) != 3 || std::fread (size3, 4, 3, f) != 3) return fail ("truncated octree header");
+  c.integrate_color = rgb ? 1 : 0;
+  for (int i = 0; i < 16; ++i) c.global_transform[i] = gt[i];
+  return B200TSDF_OK;
+}
+
+// the host loader: one record at a time, recursively, into a host image of the volume
 struct VolLoader
 {
   std::FILE* f; bool rgb; const Params* p; bool bad = false; std::string why;
-  // host image of the volume being rebuilt
+  unsigned long long ood = 0;                  // stored {d, w} outside the fast route's domain (edit_in_fast_domain)
   std::vector<float2> root_dw; std::vector<uint32_t> root_split; std::vector<uchar4> root_rgb; std::vector<float> root_M; std::vector<int> root_ns;
   std::vector<uint64_t> keys; std::vector<float2> nodes; std::vector<uint32_t> split; std::vector<uchar4> rgbv; std::vector<float> Mv; std::vector<int> nsv;
   std::unordered_map<uint64_t, int> index;
@@ -2821,70 +3097,39 @@ struct VolLoader
     const Params& P = *p;
     if (level < P.C && nchild != 8) { bad = true; why = "tree is shallower than the coarse depth implied by max_cell_size"; return; }
     if (level > P.L || (level == P.L && nchild)) { bad = true; why = "tree is deeper than the resolution"; return; }
-    if (level >= P.Rtop)
+    const VolPlace o = vol_place (P, level, x, y, z, nchild != 0);
+    if (o.stored)
     {
-      if (level == P.Rtop)
+      if (!edit_in_fast_domain (v[0], v[1])) ++ood;
+      if (o.root)
       {
-        int ri = root_index (P, x, y, z);
+        const int ri = o.root_idx;
         root_dw[ri] = make_float2 (v[0], v[1]); root_rgb[ri] = make_uchar4 (c3[0], c3[1], c3[2], 0); root_M[ri] = v[6]; root_ns[ri] = nsamp;
-        if (nchild && level >= P.C) root_split[ri >> 5] |= 1u << (ri & 31);
+        if (o.set_split) root_split[o.word] |= o.mask;
       }
       else
       {
-        int t = tier_of_level (P, level), k = level - tier_root_level (P, t);
-        int b = brick_of (t, x >> k, y >> k, z >> k);
-        int j = path_index (k, x, y, z), idx = node_offset (k) + j;
-        size_t o = (size_t) b * BRICK_NODES + idx;
-        nodes[o] = make_float2 (v[0], v[1]); rgbv[o] = make_uchar4 (c3[0], c3[1], c3[2], 0); Mv[o] = v[6]; nsv[o] = nsamp;
-        if (nchild && level >= P.C && level < P.L) split[(size_t) b * BRICK_SPLIT_WORDS + split_word_base (k) + (j >> 5)] |= 1u << (j & 31);
+        const int b = brick_of (o.t, o.bx, o.by, o.bz);
+        const size_t k = (size_t) b * BRICK_NODES + o.idx;
+        nodes[k] = make_float2 (v[0], v[1]); rgbv[k] = make_uchar4 (c3[0], c3[1], c3[2], 0); Mv[k] = v[6]; nsv[k] = nsamp;
+        if (o.set_split) split[(size_t) b * BRICK_SPLIT_WORDS + o.word] |= o.mask;
       }
     }
     for (size_t c = 0; c < nchild; ++c) node (level + 1, 2 * x + (int) ((c >> 2) & 1), 2 * y + (int) ((c >> 1) & 1), 2 * z + (int) (c & 1));
   }
 };
-}
 
-int b200tsdf_load (b200tsdf_t* h, const char* path)
+// the body at f through the host loader into the freshly reset volume; `name` prefixes the message of a malformed body
+int load_host_body (b200tsdf* h, std::FILE* f, bool rgb, const std::string& name, unsigned long long& ood)
 {
-  if (!h || !path) return B200TSDF_EINVAL;
-  std::FILE* f = std::fopen (path, "rb");
-  if (!f) return h->fail (B200TSDF_EIO, std::string ("cannot open ") + path);
-  b200tsdf_config c = h->cfg_pending;
-  char line[1024];
-  auto fail = [&] (const std::string& m) { std::fclose (f); return h->fail (B200TSDF_EIO, std::string (path) + ": " + m); };
-  if (!std::fgets (line, sizeof (line), f)) return fail ("empty file");
-  int is_empty = 0, wd = 0, wv = 0;
-  double gt[16];
-  int nread = std::fscanf (f, "%d %d %d %f %f %f %f %f %f %f %f %f %f %f %lf %lf %lf %lf %d %d %d %d %d",
-                           &c.xres, &c.yres, &c.zres, &c.xsize, &c.ysize, &c.zsize, &c.max_dist_pos, &c.max_dist_neg, &c.max_weight,
-                           &c.min_sensor_dist, &c.max_sensor_dist, &c.max_cell_x, &c.max_cell_y, &c.max_cell_z,
-                           &c.fx, &c.fy, &c.cx, &c.cy, &c.image_width, &c.image_height, &is_empty, &wd, &wv);
-  if (nread != 23) return fail ("bad header");
-  // the reference has no setter for these two: only a .vol written with them set turns the alternative weightings on (hpp:200-204)
-  if (wd || wv) return fail ("weight_by_depth_ / weight_by_variance_ volumes are not supported (the fusion here uses w_new = 1)");
-  char pct[8]; int rr = 0, cc = 0;
-  if (std::fscanf (f, " %1s %d %d", pct, &rr, &cc) != 3 || pct[0] != '%' || rr != 4 || cc != 4) return fail ("bad transform header");
-  for (int i = 0; i < 16; ++i) if (std::fscanf (f, "%lf", &gt[i]) != 1) return fail ("bad transform");
-  char type[64];
-  if (std::fscanf (f, "%63s", type) != 1) return fail ("missing node type");
-  bool rgb = std::string (type) == "RGB";
-  if (!rgb && std::string (type) != "NOCOLOR") return fail (std::string ("unsupported node type ") + type);
-  do { if (!std::fgets (line, sizeof (line), f)) return fail ("missing #OCTREEBINARY"); } while (!(line[0] == '#' && line[1] == 'O'));
-  size_t res3[3]; float size3[3];
-  if (std::fread (res3, sizeof (size_t), 3, f) != 3 || std::fread (size3, 4, 3, f) != 3) return fail ("truncated octree header");
-  c.integrate_color = rgb ? 1 : 0;
-  for (int i = 0; i < 16; ++i) c.global_transform[i] = gt[i];
-  h->cfg_pending = c;
-  int rc = b200tsdf_reset (h);
-  if (rc) { std::fclose (f); return rc; }
   const Params& p = h->p;
   VolLoader L; L.f = f; L.rgb = rgb; L.p = &p;
   size_t rn = h->vol.root_n;
   L.root_dw.assign (rn, make_float2 (-1.f, 0.f)); L.root_split.assign ((rn + 31) / 32, 0u);
   L.root_rgb.assign (rn, make_uchar4 (0, 0, 0, 0)); L.root_M.assign (rn, 0.f); L.root_ns.assign (rn, 0);
   L.node (0, 0, 0, 0);
-  std::fclose (f);
-  if (L.bad) return h->fail (B200TSDF_EIO, std::string (path) + ": " + L.why);
+  if (L.bad) return h->fail (B200TSDF_EIO, name + ": " + L.why);
+  ood = L.ood;
   cudaSetDevice (h->device);
   CK (cudaMemcpy (p.root_dw, L.root_dw.data (), rn * sizeof (float2), cudaMemcpyHostToDevice));
   CK (cudaMemcpy (p.root_split, L.root_split.data (), L.root_split.size () * sizeof (uint32_t), cudaMemcpyHostToDevice));
@@ -2901,10 +3146,209 @@ int b200tsdf_load (b200tsdf_t* h, const char* path)
     k_load_bricks<<<nb, 128, 0, s>>> (p, dk, nb, dn, ds, dc, dM, dns);
     CK (cudaStreamSynchronize (s));
   }
+  return B200TSDF_OK;
+}
+
+// The parallel parser: the body (len bytes of device memory) into the freshly reset volume.  1 when every check held and the
+// records are placed; 0 when one failed or its work space cannot be allocated, with the volume untouched (the caller runs the
+// host loader on the same bytes); < 0 on a CUDA error.
+int load_device_body (b200tsdf* h, const unsigned char* d_body, size_t len, bool rgb, unsigned long long& ood)
+{
+  const int rb = vol_record_bytes (rgb, false);
+  const size_t nrec = len / rb;
+  if (!nrec || nrec >= ((size_t) 1 << 31)) return 0;
+  cudaStream_t s = h->stream;
+  DevBuf<long long> delta (s), incl (s);
+  DevBuf<unsigned long long> res (s);
+  if (delta.alloc (nrec) || incl.alloc (nrec) || res.alloc (3)) { cudaGetLastError (); return 0; }
+  const unsigned long long init[3] = { ~0ull, 0ull, 0ull };
+  CK (cudaMemcpyAsync (res, init, sizeof (init), cudaMemcpyHostToDevice, s));
+  const unsigned blocks = (unsigned) ((nrec + 255) / 256);
+  k_vol_slots<<<blocks, 256, 0, s>>> (d_body, nrec, rb, delta);
+  CK (cudaGetLastError ());
+  const int e = b2_inclusive_sum (s, delta, incl, nrec);
+  if (e == (int) cudaErrorMemoryAllocation) { cudaGetLastError (); return 0; }
+  if (e) return h->fail (B200TSDF_ECUDA, std::string ("vol parse scan: ") + cudaGetErrorString ((cudaError_t) e));
+  k_vol_end<<<blocks, 256, 0, s>>> (incl, nrec, res);
+  unsigned long long out[3];
+  CK (cudaMemcpyAsync (out, res, sizeof (out), cudaMemcpyDeviceToHost, s));
+  CK (cudaStreamSynchronize (s));
+  if (out[0] == ~0ull) return 0;                             // the tree does not close inside the body
+  const size_t n = (size_t) out[0] + 1;
+  const unsigned nblocks = (unsigned) ((n + 255) / 256);
+  k_vol_check<<<nblocks, 256, 0, s>>> (h->p, d_body, n, rb, rgb ? 1 : 0, res);
+  CK (cudaMemcpyAsync (out, res, sizeof (out), cudaMemcpyDeviceToHost, s));
+  CK (cudaStreamSynchronize (s));
+  if (out[1]) return 0;
+  ood = out[2];
+  k_vol_place<<<nblocks, 256, 0, s>>> (h->p, d_body, n, rb, rgb ? 1 : 0);
+  CK (cudaGetLastError ());
+  return 1;
+}
+
+// after a body is in: isEmpty from the header, the fast route only for values fusion produces, and the device error bits
+int load_finish (b200tsdf* h, int is_empty, unsigned long long ood, bool on_device)
+{
   h->is_empty = is_empty != 0;
+  h->loaded_on_device = on_device;
+  if (ood && h->fast_path)
+  {
+    h->fast_path = false; h->top_path = false;
+    drop_batch_graphs (h);                                   // the captured launches take the fast route
+  }
   return check_device_err (h);
 }
 
+} // namespace
+
+extern "C" {
+
+// save (tsdf_volume_octree.cpp:222-245; Octree::serialize octree.cpp:645-657; serializeASCII
+// eigen_extensions.h:249-257)
+int b200tsdf_save (b200tsdf_t* h, const char* path)
+{
+  if (!h || !path) return B200TSDF_EINVAL;
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "save before reset()");
+  cudaSetDevice (h->device);
+  return (h->cfg_pending.debug_flags & VOL_HOST_IO) ? save_host (h, path) : save_device_file (h, path);
+}
+
+int b200tsdf_save_device (b200tsdf_t* h, void* d_buf, size_t capacity, size_t* nbytes)
+{
+  if (!h || !nbytes) return B200TSDF_EINVAL;
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "save before reset()");
+  cudaSetDevice (h->device);
+  if (int rc = b200tsdf_sync (h)) return rc;
+  const std::string hd = vol_header (h);
+  const size_t rb = (size_t) vol_record_bytes (h->p.color != 0, h->p.color_norm != 0);
+  cudaStream_t s = h->stream;
+  DevBuf<VolNode> nodes (s);
+  unsigned long long count = 0;
+  auto admit = [&] (unsigned long long n, bool& go)
+  {
+    const size_t need = hd.size () + (size_t) n * rb;
+    *nbytes = need;
+    if (!d_buf) return (int) B200TSDF_OK;
+    if (capacity < need) return h->fail (B200TSDF_EINVAL, "save buffer too small");
+    go = true;
+    return (int) B200TSDF_OK;
+  };
+  if (int rc = vol_walk (h, nodes, count, admit)) return rc;
+  if (!d_buf) return B200TSDF_OK;
+  unsigned char* o = (unsigned char*) d_buf;
+  CK (cudaMemcpyAsync (o, hd.data (), hd.size (), cudaMemcpyHostToDevice, s));
+  vol_format_launch (h, nodes, 0, (size_t) count, o + hd.size ());
+  CK (cudaGetLastError ());
+  CK (cudaStreamSynchronize (s));
+  return B200TSDF_OK;
+}
+
+int b200tsdf_load (b200tsdf_t* h, const char* path)
+{
+  if (!h || !path) return B200TSDF_EINVAL;
+  File f (std::fopen (path, "rb"));
+  if (!f) return h->fail (B200TSDF_EIO, std::string ("cannot open ") + path);
+  b200tsdf_config c; bool rgb = false; int is_empty = 0;
+  if (int rc = vol_read_header (h, f, path, c, rgb, is_empty)) return rc;
+  h->cfg_pending = c;
+  if (int rc = b200tsdf_reset (h)) return rc;
+  cudaSetDevice (h->device);
+  unsigned long long ood = 0;
+  if (!(h->cfg.debug_flags & VOL_HOST_IO))
+  {
+    // the body to the device in one buffer: the fread of each chunk overlaps the H2D copy of the one before.  When the
+    // buffers cannot be had, the host loader reads the file as it did before there was a device parser.
+    const long body = std::ftell (f);
+    std::fseek (f, 0, SEEK_END);
+    const long end = std::ftell (f);
+    std::fseek (f, body, SEEK_SET);
+    const size_t len = (body >= 0 && end > body) ? (size_t) (end - body) : 0;
+    const size_t chunk = std::max<size_t> (1, std::min (VOL_LOAD_CHUNK, len));
+    cudaStream_t s = h->stream;
+    DevBuf<unsigned char> d_body (s);
+    Pinned<unsigned char> pin[2];
+    Event ev[2];
+    bool staged = d_body.alloc (len) == cudaSuccess;
+    for (int k = 0; k < 2 && len && staged; ++k)
+    {
+      staged = pin[k].alloc (chunk) == cudaSuccess;
+      if (staged) CK (cudaEventCreateWithFlags (&ev[k].x, cudaEventDisableTiming));
+    }
+    if (!staged) cudaGetLastError ();
+    size_t got = 0;
+    for (size_t k = 0; staged && got < len; ++k)
+    {
+      const int b = (int) (k & 1);
+      if (k >= 2) CK (cudaEventSynchronize (ev[b]));
+      const size_t want = std::min (chunk, len - got);
+      const size_t r = std::fread (pin[b], 1, want, f);
+      if (r) { CK (cudaMemcpyAsync (d_body.p + got, pin[b], r, cudaMemcpyHostToDevice, s)); CK (cudaEventRecord (ev[b], s)); }
+      got += r;
+      if (r < want) break;
+    }
+    const int r = staged ? load_device_body (h, d_body, got, rgb, ood) : 0;
+    if (r < 0) return r;
+    if (r == 1) return load_finish (h, is_empty, ood, true);
+    std::fseek (f, body, SEEK_SET);
+  }
+  if (int rc = load_host_body (h, f, rgb, path, ood)) return rc;
+  return load_finish (h, is_empty, ood, false);
+}
+
+int b200tsdf_load_path (b200tsdf_t* h, int32_t* on_device)
+{
+  if (!h || !on_device) return B200TSDF_EINVAL;
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "load path before reset()");
+  *on_device = h->loaded_on_device ? 1 : 0;
+  return B200TSDF_OK;
+}
+
+int b200tsdf_load_device (b200tsdf_t* h, const void* d_buf, size_t nbytes)
+{
+  if (!h || (!d_buf && nbytes)) return B200TSDF_EINVAL;
+  const std::string name = "device image";
+  if (!nbytes) return h->fail (B200TSDF_EIO, name + ": empty file");
+  cudaSetDevice (h->device);
+  const unsigned char* d = (const unsigned char*) d_buf;
+  // the header through the same stdio code as a file: fmemopen over a host copy of the image's first bytes, or of the whole
+  // image when the header does not end well inside them
+  std::vector<unsigned char> head (std::min (nbytes, VOL_HEAD_PROBE));
+  b200tsdf_config c; bool rgb = false; int is_empty = 0;
+  long body = 0;
+  for (;;)
+  {
+    CK (cudaMemcpy (head.data (), d, head.size (), cudaMemcpyDeviceToHost));
+    File f (fmemopen (head.data (), head.size (), "rb"));
+    if (!f) return h->fail (B200TSDF_EIO, name + ": cannot open the header copy");
+    const int rc = vol_read_header (h, f, name, c, rgb, is_empty);
+    body = rc ? 0 : std::ftell (f);
+    const bool whole = head.size () == nbytes;
+    if (whole || (!rc && body >= 0 && (size_t) body + 1 < head.size ()))
+    {
+      if (rc) return rc;
+      break;
+    }
+    head.resize (nbytes);
+  }
+  h->cfg_pending = c;
+  if (int rc = b200tsdf_reset (h)) return rc;
+  cudaSetDevice (h->device);
+  unsigned long long ood = 0;
+  if (!(h->cfg.debug_flags & VOL_HOST_IO))
+  {
+    const int r = load_device_body (h, d + body, nbytes - (size_t) body, rgb, ood);
+    if (r < 0) return r;
+    if (r == 1) return load_finish (h, is_empty, ood, true);
+  }
+  const size_t blen = nbytes - (size_t) body;
+  std::vector<unsigned char> host (std::max<size_t> (blen, 1));
+  if (blen) CK (cudaMemcpy (host.data (), d + body, blen, cudaMemcpyDeviceToHost));
+  File f (fmemopen (host.data (), host.size (), "rb"));
+  if (!f) return h->fail (B200TSDF_EIO, name + ": cannot open the body copy");
+  if (!blen) std::fseek (f, 0, SEEK_END);                    // (fmemopen takes no empty buffer)
+  if (int rc = load_host_body (h, f, rgb, name, ood)) return rc;
+  return load_finish (h, is_empty, ood, false);
+}
 
 // ---- shard export / import ------------------------------------------------------------------------------------
 namespace {

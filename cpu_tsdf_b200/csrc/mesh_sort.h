@@ -14,6 +14,10 @@
 int b2_sort_records (cudaStream_t s, size_t n, int key_bits, unsigned long long* d_keys, int words, const void* d_v, const unsigned char* d_c,
                      void* d_v_out, unsigned char* d_c_out);
 
+// d_out[i] = d_in[0] + ... + d_in[i] (n < 2^31), used by the .vol parser (engine.cu).  Returns 0 or a cudaError_t with the
+// stream synchronised.
+int b2_inclusive_sum (cudaStream_t s, const long long* d_in, long long* d_out, size_t n);
+
 // Device scratch of one post-processing call: every allocation is released with the object.  The routines below end with
 // their stream synchronised, so nothing still reads it then.
 struct B2MeshScratch

@@ -423,6 +423,20 @@ __global__ void k_gather_records (const unsigned int* __restrict__ order, size_t
 }
 }
 
+int b2_inclusive_sum (cudaStream_t s, const long long* d_in, long long* d_out, size_t n)
+{
+  if (!n) return 0;
+  if (n >= ((size_t) 1 << 31)) return (int) cudaErrorInvalidValue;
+  void* tmp = nullptr;
+  size_t bytes = 0;
+  cudaError_t e = cub::DeviceScan::InclusiveSum (nullptr, bytes, d_in, d_out, (int) n, s);
+  if (e == cudaSuccess) e = cudaMalloc (&tmp, bytes);
+  if (e == cudaSuccess) e = cub::DeviceScan::InclusiveSum (tmp, bytes, d_in, d_out, (int) n, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize (s);
+  cudaFree (tmp);
+  return (int) e;
+}
+
 int b2_sort_records (cudaStream_t s, size_t ntri, int key_bits, unsigned long long* d_keys, int words, const void* d_v, const unsigned char* d_c,
                      void* d_v_out, unsigned char* d_c_out)
 {

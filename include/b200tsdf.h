@@ -54,7 +54,8 @@ typedef struct b200tsdf_config
   int32_t device;                           /* CUDA device ordinal                                */
   int32_t pool_log2;                        /* brick pool capacity = 2^pool_log2 (0 = default 20) */
   int32_t shard_rank, shard_count;          /* this handle owns coarse cells with hash(cell) % shard_count == shard_rank */
-  int32_t debug_flags;                      /* bit0: general depth-first update kernel only; bit1: per-level upper sweeps instead of the fused per-cell ones; other bits are ignored */
+  int32_t debug_flags;                      /* bit0: general depth-first update kernel only; bit1: per-level upper sweeps instead of the fused per-cell ones;
+                                               bit2: .vol save and load through the host writer and loader; other bits are ignored */
   int32_t color_mode;                       /* setColorMode (tsdf_volume_octree.h:290) — B200TSDF_COLOR_RGB (default) or B200TSDF_COLOR_RGB_NORMALIZED
                                                (octree.cpp:379-434; fused by the general kernel).  "LAB" (octree.cpp:436-581) is refused: RGB2LAB needs libm pow */
   int32_t reserved[2];
@@ -252,6 +253,25 @@ int  b200tsdf_save (b200tsdf_t* h, const char* path);
  * (resolution, size, truncation, intrinsics, ..., colour node type) and rebuilds the volume on the device.
  * OctreeNode::M_/nsample_ are kept only if track_variance was set on the handle. */
 int  b200tsdf_load (b200tsdf_t* h, const char* path);
+
+/* .vol images in device memory (DESIGN.md §3e).  b200tsdf_save_device writes the whole file image that b200tsdf_save would
+ * write (header and body, byte for byte) into d_buf, device memory of the handle's device, and sets *nbytes to its size.
+ * d_buf == NULL only sets *nbytes; capacity < *nbytes returns B200TSDF_EINVAL with nothing written.  Ordered after every
+ * integrate queued on the handle; returns once the image is written.  B200TSDF_ESTATE before reset(), B200TSDF_ENOMEM when
+ * the node records or their sort do not fit.
+ * b200tsdf_load_device (h, d_buf, nbytes) is b200tsdf_load of a file holding those nbytes bytes: the same configuration,
+ * volume, result codes and messages (the messages name the "device image" instead of a path).
+ * Both loaders parse the body on the device when every record of it is where the reference's writer would put it, and
+ * otherwise, or when the parser's work space cannot be allocated, run the host loader on the same bytes; bytes after the
+ * tree are ignored.  A file holding a {d, w} that fusion does
+ * not produce (|d| > 2^38, w < 0, w = -0, 0 < w < 1e-20 or w > 2^38) moves later integrates to the general kernel until the
+ * next b200tsdf_reset or load, as b200tsdf_set_containing_voxels does. */
+int  b200tsdf_save_device (b200tsdf_t* h, void* d_buf, size_t capacity, size_t* nbytes);
+int  b200tsdf_load_device (b200tsdf_t* h, const void* d_buf, size_t nbytes);
+/* *on_device = 1 when the last b200tsdf_load / b200tsdf_load_device placed the file's body with the device parser, 0 when the
+ * host loader did (debug_flags bit 2, a file no writer produces, or parser work space that could not be allocated) or when
+ * the volume comes from b200tsdf_reset.  B200TSDF_ESTATE before reset(). */
+int  b200tsdf_load_path (b200tsdf_t* h, int32_t* on_device);
 
 /* Shard gather (multi-GPU, DESIGN.md §5): a handle created with shard_count > 1 owns the coarse cells with
  * hash(cell) % shard_count == shard_rank.  b200tsdf_export_shard serialises everything this handle owns (the

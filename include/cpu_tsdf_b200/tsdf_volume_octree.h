@@ -282,6 +282,17 @@ public:
   void save (const std::string& filename) const { if (h_) b200tsdf_save (h_, filename.c_str ()); }   // cpp:222-245
   void load (const std::string& filename)                                                           // cpp:248-275
   { if (h_) { status_ = b200tsdf_load (h_, filename.c_str ()); b200tsdf_get_config (h_, &cfg_); } }
+  // extension: the .vol image in device memory of the volume's device (b200tsdf_save_device / b200tsdf_load_device).
+  // saveToDevice with d_buf == nullptr sets *nbytes only; both return a B200TSDF_ code.
+  int saveToDevice (void* d_buf, std::size_t capacity, std::size_t* nbytes) const
+  { return h_ ? b200tsdf_save_device (h_, d_buf, capacity, nbytes) : B200TSDF_ESTATE; }
+  int loadFromDevice (const void* d_buf, std::size_t nbytes)
+  {
+    if (!h_) return B200TSDF_ESTATE;
+    status_ = b200tsdf_load_device (h_, d_buf, nbytes);
+    b200tsdf_get_config (h_, &cfg_);
+    return status_;
+  }
 
   PointXYZ getVoxelCenter (std::size_t x, std::size_t y, std::size_t z) const                      // cpp:553-560
   { float o[3] = { 0, 0, 0 }; b200tsdf_voxel_center (h_, (std::int64_t) x, (std::int64_t) y, (std::int64_t) z, o); PointXYZ p; p.x = o[0]; p.y = o[1]; p.z = o[2]; return p; }
