@@ -70,7 +70,7 @@ class OrganizeOpts(C.Structure):
 
 EXPORTS = [
     "b200tsdf_default_config", "b200tsdf_create", "b200tsdf_destroy", "b200tsdf_last_error",
-    "b200tsdf_set_config", "b200tsdf_get_config", "b200tsdf_reset", "b200tsdf_integrate",
+    "b200tsdf_set_config", "b200tsdf_get_config", "b200tsdf_reset", "b200tsdf_resize_pool", "b200tsdf_integrate",
     "b200tsdf_integrate_device", "b200tsdf_integrate_batch_device", "b200tsdf_integrate_async",
     "b200tsdf_comm_unique_id", "b200tsdf_comm_init", "b200tsdf_row_slice", "b200tsdf_integrate_batch_rows", "b200tsdf_gather_volume", "b200tsdf_sync", "b200tsdf_organize", "b200tsdf_integrate_unorganized", "b200tsdf_integrate_unorganized_batch_device", "b200tsdf_query", "b200tsdf_interpolate", "b200tsdf_render", "b200tsdf_mesh",
     "b200tsdf_query_device", "b200tsdf_interpolate_device", "b200tsdf_render_batch_device",
@@ -118,6 +118,7 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_set_config.argtypes = [vp, C.POINTER(Config)]
     lib.b200tsdf_get_config.argtypes = [vp, C.POINTER(Config)]
     lib.b200tsdf_reset.argtypes = [vp]
+    lib.b200tsdf_resize_pool.argtypes = [vp, C.c_int]
     lib.b200tsdf_integrate.argtypes = [vp, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, vp]
     lib.b200tsdf_integrate_device.argtypes = [vp, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, vp]
     lib.b200tsdf_integrate_async.argtypes = [vp, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_int, vp]
@@ -297,6 +298,14 @@ class TSDFVolumeOctree:
     def reset(self):
         """tsdf_volume_octree.cpp:201-219"""
         self._check(self._lib.b200tsdf_reset(self._h))
+
+    def resizePool(self, pool_log2: int):
+        """(no counterpart) Move the live volume into a brick pool of 2^pool_log2 bricks, on the device.  Integration goes on
+        bit for bit as if the volume had been reset with that pool.  Refused (B200Error, nothing changed) when the claimed
+        bricks exceed 7/8 of the new pool (stats().n_bricks against the capacity), when the new pool cannot be allocated
+        (the old and the new pool coexist while the bricks move), and when an earlier call left an error latched."""
+        self._check(self._lib.b200tsdf_resize_pool(self._h, int(pool_log2)))
+        self._check(self._lib.b200tsdf_get_config(self._h, C.byref(self._cfg)))
 
     def integrateCloud(self, cloud: np.ndarray, normals=None, trans=np.eye(4)) -> bool:
         """impl/tsdf_volume_octree.hpp:48-103 (normals are unused there as well)."""

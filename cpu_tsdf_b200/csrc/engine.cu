@@ -13,6 +13,7 @@
 #include "mesh_sort.h"
 #include "host_pack.h"
 #include "vol_io.cuh"
+#include "pool_rehash.cuh"
 
 #include <cuda_runtime.h>
 #include <sys/mman.h>
@@ -549,6 +550,20 @@ __global__ void k_load_bricks (Params p, const uint64_t* __restrict__ keys, int 
     if (p.M && M) { p.M[s * BRICK_NODES + i] = M[(size_t) b * BRICK_NODES + i]; p.ns[s * BRICK_NODES + i] = ns[(size_t) b * BRICK_NODES + i]; }
   }
   for (int i = threadIdx.x; i < BRICK_SPLIT_WORDS; i += blockDim.x) p.split[s * BRICK_SPLIT_WORDS + i] = split[(size_t) b * BRICK_SPLIT_WORDS + i];
+}
+
+// b200tsdf_resize_pool: the claimed old slots in list[0, n) into the fresh pool of `to`, one warp per brick (REHASH_THREADS / 32
+// bricks per CTA).  A brick that finds no slot within MAX_PROBE raises ERR_POOL_FULL on to.err and is dropped.
+constexpr int REHASH_THREADS = 256;
+__global__ void __launch_bounds__ (REHASH_THREADS) k_pool_rehash (Params from, Params to, const int* __restrict__ list, int n)
+{
+  const int b = (int) ((blockIdx.x * (unsigned) REHASH_THREADS + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (b >= n) return;
+  const uint32_t s = (uint32_t) list[b];
+  int d = 0;
+  if (lane == 0) d = rehash_claim (from, to, s);
+  d = __shfl_sync (0xffffffffu, d, 0);
+  if (d >= 0) rehash_brick (from, to, s, (uint32_t) d, lane, 32);
 }
 
 // shard import: scatter coarse-cell (root array) entries
@@ -1131,6 +1146,22 @@ int alloc_failed (b200tsdf* h, const std::string& what)
   return h->fail (B200TSDF_ENOMEM, "device allocation failed (" + what + ")");
 }
 
+// Every brick slot of the pool q points at (pool slots) fresh, by the invariant of tsdf_core.cuh (OctreeNode ctor: d=-1, w=0;
+// octree.h:71-74): no key, no split bit, zero colour / variance payload and work byte.  Enqueued on the handle's stream.
+int fresh_pool (b200tsdf* h, const Params& q, size_t pool)
+{
+  cudaStream_t s = h->stream;
+  const size_t nn = pool * BRICK_NODES;
+  CK (cudaMemsetAsync (q.keys, 0, pool * sizeof (uint64_t), s));
+  CK (cudaMemsetAsync (q.split, 0, pool * BRICK_SPLIT_WORDS * sizeof (uint32_t), s));
+  CK (cudaMemsetAsync (q.work, 0, pool, s));
+  k_fill_fresh<<<h->sm_count * 8, 256, 0, s>>> (q.nodes, nn);
+  if (q.rgb) CK (cudaMemsetAsync (q.rgb, 0, nn * sizeof (uchar4), s));
+  if (q.M) { CK (cudaMemsetAsync (q.M, 0, nn * sizeof (float), s)); CK (cudaMemsetAsync (q.ns, 0, nn * sizeof (int), s)); }
+  if (q.rgbn) CK (cudaMemsetAsync (q.rgbn, 0, nn * sizeof (float4), s));
+  return B200TSDF_OK;
+}
+
 // `bytes` of device memory into `host` (reallocated with malloc, at least one byte), after the work queued before them
 int download (b200tsdf* h, const void* d, size_t bytes, void*& host)
 {
@@ -1368,16 +1399,11 @@ int b200tsdf_reset (b200tsdf_t* h)
   CK (cudaStreamSynchronize (h->stream));                            // (&p is host memory that may change after reset)
   // fresh state everywhere (OctreeNode ctor: d=-1, w=0; octree.h:71-74)
   cudaStream_t s = h->stream;
-  CK (cudaMemsetAsync (p.keys, 0, pool * sizeof (uint64_t), s));
-  CK (cudaMemsetAsync (p.split, 0, pool * BRICK_SPLIT_WORDS * sizeof (uint32_t), s));
-  CK (cudaMemsetAsync (p.work, 0, pool, s));
-  k_fill_fresh<<<h->sm_count * 8, 256, 0, s>>> (p.nodes, pool * BRICK_NODES);
-  if (color) CK (cudaMemsetAsync (p.rgb, 0, pool * BRICK_NODES * sizeof (uchar4), s));
-  if (var) { CK (cudaMemsetAsync (p.M, 0, pool * BRICK_NODES * sizeof (float), s)); CK (cudaMemsetAsync (p.ns, 0, pool * BRICK_NODES * sizeof (int), s)); }
+  if (int rc = fresh_pool (h, p, pool)) return rc;
   k_fill_fresh<<<64, 256, 0, s>>> (p.root_dw, root_n);
   CK (cudaMemsetAsync (p.root_split, 0, ((root_n + 31) / 32) * sizeof (uint32_t), s));
   if (color) CK (cudaMemsetAsync (p.root_rgb, 0, root_n * sizeof (uchar4), s));
-  if (norm) { CK (cudaMemsetAsync (p.rgbn, 0, pool * BRICK_NODES * sizeof (float4), s)); CK (cudaMemsetAsync (p.root_rgbn, 0, root_n * sizeof (float4), s)); }
+  if (norm) CK (cudaMemsetAsync (p.root_rgbn, 0, root_n * sizeof (float4), s));
   if (var) { CK (cudaMemsetAsync (p.root_M, 0, root_n * sizeof (float), s)); CK (cudaMemsetAsync (p.root_ns, 0, root_n * sizeof (int), s)); }
   CK (cudaMemsetAsync (h->d_err, 0, sizeof (int), s));
   *h->h_err = 0;
@@ -1398,6 +1424,73 @@ int b200tsdf_reset (b200tsdf_t* h)
   h->loaded_on_device = false;
   h->has_volume = true;
   return check_device_err (h);
+}
+
+// ---- resizing the brick pool of a live volume (DESIGN.md §3f) ----------------------------------------
+// Every claimed brick is rehashed into a fresh pool of the new size, next to the old one, which is freed only once the new one
+// holds every brick.  Like reset (), the handle takes the new storage in one step at the end: a refusal or a failed allocation
+// leaves it as it was.
+int b200tsdf_resize_pool (b200tsdf_t* h, int pool_log2)
+{
+  if (!h) return B200TSDF_EINVAL;
+  cudaSetDevice (h->device);
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "resize_pool before reset()");
+  CK (cudaStreamSynchronize (h->copy_stream));
+  CK (cudaStreamSynchronize (h->gather_stream));
+  int e = 0;
+  CK (cudaMemcpyAsync (&e, h->d_err, sizeof (int), cudaMemcpyDeviceToHost, h->stream));
+  CK (cudaStreamSynchronize (h->stream));
+  if (e || h->half_launched)
+    return h->fail (B200TSDF_ESTATE, "resize_pool on a volume with an error latched by an earlier call; reset() the handle");
+  const size_t pool = pool_capacity_of (pool_log2);
+  if (!pool) return h->fail (B200TSDF_EINVAL, "pool_log2 out of range [8,26]");
+  int* list = nullptr;
+  const int nb = list_bricks (h, list);
+  if (nb < 0) return nb;
+  if (!rehash_fits (nb, (long long) pool))
+    return h->fail (B200TSDF_EINVAL, "resize_pool: " + std::to_string (nb) + " bricks do not fit a pool of " + std::to_string (pool)
+                                     + " at the load limit of 7/8");
+
+  // the new pool, fresh, beside the old one
+  const Volume& v = h->vol;
+  Volume nv;
+  const size_t nn = pool * BRICK_NODES;
+  if (nv.keys.grow (pool) || nv.nodes.grow (nn) || nv.split.grow (pool * BRICK_SPLIT_WORDS) || nv.work.grow (pool)
+      || (v.color && nv.rgb.grow (nn)) || (v.var && (nv.M.grow (nn) || nv.ns.grow (nn))) || (v.norm && nv.rgbn.grow (nn)))
+    return alloc_failed (h, "resized brick pool");
+  DevBuf<int> d_rerr (h->stream);                      // the rehash's own error bits: the handle's d_err stays as it is
+  if (d_rerr.grow (1)) return alloc_failed (h, "resize_pool error flag");
+  Params to = h->p;
+  to.keys = nv.keys; to.nodes = nv.nodes; to.split = nv.split; to.work = nv.work;
+  to.rgb = nv.rgb; to.M = nv.M; to.ns = nv.ns; to.rgbn = nv.rgbn;
+  to.pool_mask = (uint32_t) (pool - 1);
+  to.err = d_rerr;
+  cudaStream_t s = h->stream;
+  if (int rc = fresh_pool (h, to, pool)) return rc;
+  CK (cudaMemsetAsync (d_rerr, 0, sizeof (int), s));
+  if (nb) k_pool_rehash<<<(unsigned) ((nb + REHASH_THREADS / 32 - 1) / (REHASH_THREADS / 32)), REHASH_THREADS, 0, s>>> (h->p, to, list, nb);
+  CK (cudaGetLastError ());
+  int re = 0;
+  CK (cudaMemcpyAsync (&re, d_rerr, sizeof (int), cudaMemcpyDeviceToHost, s));
+  CK (cudaStreamSynchronize (s));
+  if (re & ERR_POOL_FULL)
+    return h->fail (B200TSDF_EINVAL, "resize_pool: a brick found no slot within the probe limit of the new pool; the volume is unchanged");
+
+  // install: the new pool with the old root arrays; the old pool is freed with nv
+  nv.root_dw = std::move (h->vol.root_dw); nv.root_split = std::move (h->vol.root_split); nv.root_rgb = std::move (h->vol.root_rgb);
+  nv.root_rgbn = std::move (h->vol.root_rgbn); nv.root_M = std::move (h->vol.root_M); nv.root_ns = std::move (h->vol.root_ns);
+  nv.pool = pool; nv.root_n = v.root_n; nv.color = v.color; nv.var = v.var; nv.norm = v.norm;
+  std::swap (h->vol, nv);
+  drop_batch_graphs (h);                                   // captured launches carry the old storage in their Params
+  h->storage_into (h->p);
+  h->p.pool_mask = to.pool_mask;
+  h->cfg.pool_log2 = h->cfg_pending.pool_log2 = pool_log2 > 0 ? pool_log2 : 20;
+  if (cudaMemcpyAsync (h->d_params, &h->p, sizeof (Params), cudaMemcpyHostToDevice, s) != cudaSuccess || cudaStreamSynchronize (s) != cudaSuccess)
+  {
+    h->has_volume = false;
+    return h->fail (B200TSDF_ECUDA, std::string ("resize_pool: installing the new pool failed: ") + cudaGetErrorString (cudaGetLastError ()));
+  }
+  return B200TSDF_OK;
 }
 
 // ---- integrateCloud (hpp:48-103) ------------------------------------------------------------------

@@ -15,6 +15,13 @@ inline int ilog2_exact (int v) { int l = 0; while ((1 << l) < v && l < 30) ++l; 
 // the smallest float not below t: for every float d, d < at_least (t) <=> (double) d < t (the host twin of float_at_least)
 inline float at_least (double t) { float f = (float) t; if ((double) f < t) f = std::nextafterf (f, INFINITY); return f; }
 
+// the brick pool capacity pool_log2 asks for (0 or less: the default, 2^20 bricks), or 0 outside [8, 26]
+inline size_t pool_capacity_of (int pool_log2)
+{
+  const int l = pool_log2 > 0 ? pool_log2 : 20;
+  return l < 8 || l > 26 ? 0 : (size_t) 1 << l;
+}
+
 // returns nullptr on success or a message describing the unsupported configuration
 inline const char* derive_params (const b200tsdf_config& c, Params& p, size_t& pool, size_t& root_n)
 {
@@ -36,9 +43,8 @@ inline const char* derive_params (const b200tsdf_config& c, Params& p, size_t& p
   int T = (L - C + 2) / 3;
   int Rtop = L - 3 * T;
   if (Rtop < 0) return "resolution too small for its coarse cell size: need log2(res) - 3*ceil((log2(res)-coarse)/3) >= 0";
-  int pool_log2 = c.pool_log2 > 0 ? c.pool_log2 : 20;
-  if (pool_log2 < 8 || pool_log2 > 26) return "pool_log2 out of range [8,26]";
-  pool = (size_t) 1 << pool_log2;
+  pool = pool_capacity_of (c.pool_log2);
+  if (!pool) return "pool_log2 out of range [8,26]";
   root_n = (size_t) 1 << (3 * Rtop);
   p.L = L; p.C = C; p.T = T; p.Rtop = Rtop; p.res = c.xres;
   p.size = c.xsize; p.half = c.xsize / 2; p.finest_size = c.xsize / c.xres;

@@ -79,6 +79,25 @@ int  b200tsdf_get_config (const b200tsdf_t* h, b200tsdf_config* cfg);
  * b200tsdf_load resets the handle to the file's configuration and leaves it the same way when that reset fails. */
 int  b200tsdf_reset (b200tsdf_t* h);
 
+/* (no counterpart in the reference) Moves the live volume into a brick pool of 2^pool_log2 bricks (0: the default, 2^20),
+ * on the device, so that a volume can start with a small pool and grow, or give back memory it does not use.  The call waits
+ * behind all work queued on the handle and returns once the new pool is installed.  The old and the new pool exist side by
+ * side while the bricks move: the peak device memory is the sum of both.
+ *   B200TSDF_OK: every claimed brick is in the new pool with its key, {d, w} nodes, split words, colour, RGBNormalized and
+ *     variance payload and work byte; every other slot of the new pool is fresh.  The root arrays, isEmpty, the frame
+ *     numbering and the configuration are unchanged, except that pool_log2 (b200tsdf_get_config) and pool_capacity
+ *     (b200tsdf_get_stats) report the new size.  Integration continues bit for bit as on a handle reset with that pool.
+ *     The same size as now is allowed and rehashes too.
+ *   B200TSDF_EINVAL, nothing changed: pool_log2 outside what reset() accepts ([8, 26], or 0); the claimed bricks
+ *     (b200tsdf_stats::n_bricks) above 7/8 of the new capacity, the load limit of a resize; or a brick that finds no slot
+ *     within the probe limit of the new pool.
+ *   B200TSDF_ENOMEM, nothing changed: the new pool cannot be allocated.
+ *   B200TSDF_ESTATE, nothing changed: before reset(), or when an earlier call left an error latched (a pool that overflowed
+ *     in an earlier frame, a frame left half launched): resizing does not make an incomplete volume whole; reset() it.
+ *   B200TSDF_ECUDA: a CUDA error; one while the new pool is installed leaves the handle without a volume, as reset() does.
+ * Not collective: each shard resizes its own handle, and b200tsdf_gather_volume takes shards of any pool sizes. */
+int  b200tsdf_resize_pool (b200tsdf_t* h, int pool_log2);
+
 /* TSDFVolumeOctree::integrateCloud<PointT,NormalT> (include/cpu_tsdf/impl/
  * tsdf_volume_octree.hpp:48-103).  points: organized W x H cloud in the sensor frame,
  * row-major (cloud(u,v) = points[v*W+u]), `stride` bytes per point, xyz as 3 floats at

@@ -294,6 +294,15 @@ public:
     return status_;
   }
 
+  // extension: move the live volume into a brick pool of 2^pool_log2 bricks (b200tsdf_resize_pool); sets status ()
+  bool resizePool (int pool_log2)
+  {
+    if (!h_) { status_ = B200TSDF_ENODEVICE; return false; }
+    status_ = b200tsdf_resize_pool (h_, pool_log2);
+    b200tsdf_get_config (h_, &cfg_);
+    return status_ == 0;
+  }
+
   PointXYZ getVoxelCenter (std::size_t x, std::size_t y, std::size_t z) const                      // cpp:553-560
   { float o[3] = { 0, 0, 0 }; b200tsdf_voxel_center (h_, (std::int64_t) x, (std::int64_t) y, (std::int64_t) z, o); PointXYZ p; p.x = o[0]; p.y = o[1]; p.z = o[2]; return p; }
   bool getVoxelIndex (float x, float y, float z, int& x_i, int& y_i, int& z_i) const               // cpp:562-574
