@@ -82,6 +82,7 @@ EXPORTS = [
     "b200tsdf_mesh_device", "b200tsdf_mesh_flatten_device", "b200tsdf_mesh_cleanup_device",
     "b200tsdf_containing_voxels", "b200tsdf_containing_voxels_device", "b200tsdf_dense_device",
     "b200tsdf_set_containing_voxels", "b200tsdf_set_containing_voxels_device",
+    "b200tsdf_changed_cells", "b200tsdf_mesh_cells_device",
 ]
 
 # b200tsdf_voxel (include/b200tsdf.h): one record of getContainingVoxel; level -1 = NULL
@@ -146,6 +147,8 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_render_batch_device.argtypes = [vp, C.c_int, vp, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, vp]
     lib.b200tsdf_mesh.argtypes = [vp, C.c_float, C.c_int, C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_size_t)]
     lib.b200tsdf_mesh_device.argtypes = [vp, C.c_float, C.c_int, vp, vp, C.c_size_t, szp]
+    lib.b200tsdf_mesh_cells_device.argtypes = [vp, C.c_float, C.c_int, vp, vp, vp, C.c_size_t, szp, vp]
+    lib.b200tsdf_changed_cells.argtypes = [vp, C.c_uint64, C.POINTER(C.c_uint64), vp]
     lib.b200tsdf_mesh_flatten_device.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, C.c_float, vp, vp, szp, szp]
     lib.b200tsdf_mesh_cleanup_device.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, C.c_float, C.c_int, vp, vp, szp, szp]
     lib.b200tsdf_save.argtypes = [vp, C.c_char_p]
@@ -649,6 +652,16 @@ class TSDFVolumeOctree:
         self._check(self._lib.b200tsdf_frustum_cull(self._h, _ptr(pose), _ptr(mask), _ptr(kept)))
         return mask.astype(bool)
 
+    def changedCells(self, since: int = 0):
+        """Change epochs per coarse cell (DESIGN.md §3g).  Returns (now, mask): `now` is the volume's epoch, and mask, a
+        numpy.uint8[8^C] in the layout of getFrustumCulledVoxels ((x n + y) n + z), is 1 for every cell whose mesh may differ
+        from one taken at epoch `since` (since=0: every cell).  Waits for the volume's queued work."""
+        n = 1 << (3 * self.stats().coarse_level)
+        mask = np.zeros(n, np.uint8)
+        now = C.c_uint64()
+        self._check(self._lib.b200tsdf_changed_cells(self._h, int(since), C.byref(now), _ptr(mask)))
+        return now.value, mask
+
     # -- introspection ---------------------------------------------------------------------
     def stats(self) -> Stats:
         s = Stats()
@@ -734,6 +747,154 @@ class MarchingCubesTSDFOctree:
         dp = lambda a: None if a is None else C.c_void_p(int(a))
         v._check(v._lib.b200tsdf_mesh_device(v._h, self.w_min_, mode, dp(d_verts), dp(d_rgb), int(capacity), C.byref(n)))
         return n.value
+
+    def _mode(self):
+        return 2 if self.color_by_confidence_ else (1 if self.color_by_rgb_ else 0)
+
+    def _cells_call(self, mask, d_verts, capacity, d_rgb):
+        v = self.tsdf_volume_
+        if v is None:
+            raise B200Error("setInputTSDF first")
+        ncells = 1 << (3 * v.stats().coarse_level)
+        if mask is not None:
+            mask = np.ascontiguousarray(mask, dtype=np.uint8).reshape(-1)
+            if mask.size != ncells:
+                raise ValueError(f"mask has {mask.size} entries, the volume has {ncells} coarse cells")
+        counts = np.zeros(ncells, np.int64)
+        n = C.c_size_t()
+        dp = lambda a: None if a is None else C.c_void_p(int(a))
+        rc = v._lib.b200tsdf_mesh_cells_device(v._h, self.w_min_, self._mode(), _ptr(mask), dp(d_verts), dp(d_rgb), int(capacity),
+                                               C.byref(n), _ptr(counts))
+        return rc, n.value, counts
+
+    def reconstructCellsDevice(self, mask, d_verts: int | None = None, capacity: int = 0, d_rgb: int | None = None):
+        """reconstructDevice restricted to the coarse cells with mask[c] != 0 (mask: 8^C bytes in the layout of
+        TSDFVolumeOctree.changedCells; None: every cell): the full mesh's triangles of those cells, in the same order.
+        Returns (nverts, cell_nverts), cell_nverts a numpy.int64[8^C] of each cell's vertex count (0 where not selected).
+        d_verts=None counts only; capacity and errors as reconstructDevice."""
+        rc, n, counts = self._cells_call(mask, d_verts, capacity, d_rgb)
+        self.tsdf_volume_._check(rc)
+        return n, counts
+
+
+def _morton_cells(ncells):
+    """perm[k] = the layout index ((x n + y) n + z) of the k-th coarse cell in depth-first (Morton) order, x high: the order in
+    which cells follow each other in the mesh"""
+    bits = (int(ncells).bit_length() - 1) // 3
+    k = np.arange(ncells, dtype=np.int64)
+    x = np.zeros_like(k); y = np.zeros_like(k); z = np.zeros_like(k)
+    for l in range(bits - 1, -1, -1):
+        c = (k >> (3 * l)) & 7
+        x = (x << 1) | (c >> 2); y = (y << 1) | ((c >> 1) & 1); z = (z << 1) | (c & 1)
+    n = 1 << bits
+    return (x * n + y) * n + z
+
+
+class IncrementalMesh:
+    """The mesh of a live volume, kept up to date by re-meshing only the coarse cells that changed (DESIGN.md §3g).
+
+    update() returns (verts [N,3] float32, rgb [N,3] uint8 or None) as torch tensors on the volume's device, equal bit for
+    bit to MarchingCubesTSDFOctree.reconstructDevice with the same w_min and colour mode.  Each call asks the volume which
+    cells may have changed since the last one (changedCells), meshes those cells (reconstructCellsDevice) and splices their
+    runs between the kept runs of the other cells, in Morton cell order, with one gather.  The first call, and a call after
+    w_min or color_mode changed, meshes every cell.  color_mode: 0 none, 1 RGB, 2 confidence."""
+
+    def __init__(self, volume: TSDFVolumeOctree, w_min: float = 2.5, color_mode: int = 0):
+        if color_mode not in (0, 1, 2):
+            raise ValueError("color_mode must be 0 (none), 1 (RGB) or 2 (confidence)")
+        self.volume = volume
+        self.w_min = float(w_min)
+        self.color_mode = int(color_mode)
+        self.cells_remeshed = 0          # coarse cells the last update() meshed
+        self.verts_remeshed = 0          # vertices those cells hold now
+        self._epoch = None               # the volume's epoch at the last update
+        self._made_with = None           # (w_min, color_mode) of the kept mesh
+        self._verts = self._rgb = None
+        self._cell_nverts = None         # torch.int64[8^C] on the device, in Morton order: vertices per cell of the kept mesh
+        self._host_counts = None         # the same per cell in the cell layout, on the host
+        self._buf_v = self._buf_c = None # grow-only buffers the changed cells are meshed into
+        self._morton = None              # layout index of the k-th cell in the mesh's (Morton) order, on the device
+
+    def _mesh_cells(self, mask):
+        import torch
+        mc = MarchingCubesTSDFOctree()
+        mc.setInputTSDF(self.volume)
+        mc.setMinWeight(self.w_min)
+        mc.setColorByRGB(self.color_mode == 1)
+        mc.setColorByConfidence(self.color_mode == 2)
+        dev = torch.device("cuda", self.volume._cfg.device)
+        if self.color_mode and self._buf_v is not None and self._buf_c is None:
+            self._buf_v = None
+        while True:
+            have = self._buf_v is not None
+            cap = self._buf_v.shape[0] if have else 0
+            rc, n, counts = mc._cells_call(mask, self._buf_v.data_ptr() if have else None, cap,
+                                           self._buf_c.data_ptr() if have and self.color_mode else None)
+            if rc == 0 and (have or n == 0):
+                return n, counts
+            if rc != 0 and not (have and n > cap):
+                self.volume._check(rc)
+            # no buffer yet, or one too small for these cells: grow it and mesh them again
+            cap = max(n + n // 4, 3 * 1024)
+            self._buf_v = torch.empty((cap, 3), dtype=torch.float32, device=dev)
+            self._buf_c = torch.empty((cap, 3), dtype=torch.uint8, device=dev) if self.color_mode else None
+
+    def _new_runs(self, n):
+        import torch
+        if n == 0:
+            dev = torch.device("cuda", self.volume._cfg.device)
+            return torch.empty((0, 3), dtype=torch.float32, device=dev), torch.empty((0, 3), dtype=torch.uint8, device=dev)
+        return self._buf_v[:n], (self._buf_c[:n] if self.color_mode else None)
+
+    def update(self):
+        import torch
+        vol = self.volume
+        made_with = (self.w_min, self.color_mode)
+        full = self._epoch is None or made_with != self._made_with
+        now, mask = vol.changedCells(0 if full else self._epoch)
+        sel = np.flatnonzero(mask)
+        dev = torch.device("cuda", vol._cfg.device)
+        if full or len(sel) == mask.size:
+            n, counts = self._mesh_cells(None)
+            new_v, new_c = self._new_runs(n)
+            self._verts = new_v.clone()
+            self._rgb = new_c.clone() if self.color_mode else None
+            if self._morton is None or self._morton.numel() != mask.size:
+                self._morton = torch.from_numpy(_morton_cells(mask.size)).to(dev)
+            self._cell_nverts = torch.from_numpy(counts).to(dev)[self._morton]
+            self._host_counts = counts
+        elif len(sel):
+            n, counts = self._mesh_cells(mask)
+            new_v, new_c = self._new_runs(n)
+            if self._morton is None or self._morton.numel() != mask.size:
+                self._morton = torch.from_numpy(_morton_cells(mask.size)).to(dev)
+            perm = self._morton
+            # every per-cell array below is in the mesh's cell order (Morton), where each cell's run is contiguous
+            new_counts = torch.from_numpy(counts).to(dev)[perm]
+            sel_t = torch.from_numpy(mask.astype(bool)).to(dev)[perm]
+            old_counts = self._cell_nverts
+            cell_nverts = torch.where(sel_t, new_counts, old_counts)
+            total = int(np.where(mask != 0, counts, self._host_counts).sum())
+            zero = torch.zeros(1, dtype=torch.int64, device=dev)
+            excl = lambda c: torch.cat((zero, torch.cumsum(c, 0)[:-1]))
+            n_old = self._verts.shape[0]
+            # source of cell c's run in cat(old mesh, new runs): its old run, or its new run behind the old mesh
+            base = torch.where(sel_t, n_old + excl(new_counts), excl(old_counts))
+            out_off = excl(cell_nverts)
+            cell = torch.repeat_interleave(torch.arange(cell_nverts.numel(), device=dev), cell_nverts, output_size=total)
+            idx = base[cell] + torch.arange(total, device=dev) - out_off[cell]
+            self._verts = torch.cat((self._verts, new_v))[idx]
+            if self.color_mode:
+                self._rgb = torch.cat((self._rgb, new_c))[idx]
+            self._cell_nverts = cell_nverts
+            self._host_counts = np.where(mask != 0, counts, self._host_counts)
+        else:
+            n = 0
+        self.cells_remeshed = int(len(sel)) if not full else int(mask.size)
+        self.verts_remeshed = int(n)
+        self._epoch = now
+        self._made_with = made_with
+        return self._verts, self._rgb
 
 
 # ---- mesh post-processing of the reference's `integrate` program (src/prog/integrate.cpp:103-214) ----------

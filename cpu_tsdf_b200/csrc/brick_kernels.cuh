@@ -39,6 +39,7 @@ struct FrameRec
   int timing;              // 1: the brick kernel stamps kt[] with %globaltimer (profiling; works inside a replayed graph)
   uint32_t seq;            // the frame's sequence number on its handle (the value of its fold marks, see FoldState)
   int gated;               // 1: k_front waits per supercell for the previous frame's fold instead of for its whole last kernel
+  unsigned long long epoch;// the frame's epoch on its handle: k_front stamps the cells it may change with it (Params::cell_epoch)
   unsigned long long kt[2];// [0] start of the brick kernel (ns), [1] end of its last block; zeroed by the record upload
 };
 // programmatic dependent launch: the hot kernels of a frame are launched with programmatic stream serialization, so the next

@@ -170,6 +170,15 @@ __global__ void k_cull (Params p, Planes P, unsigned char* __restrict__ mask)
   mask[i] = frustum_contains (P.pl, cx, cy, cz) ? 1 : 0;
 }
 
+// b200tsdf_changed_cells: the mask of cell_changed over the 8^C cells
+__global__ void k_changed_cells (int C, const unsigned long long* __restrict__ cell_epoch, unsigned long long since,
+                                 unsigned char* __restrict__ mask)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 1 << (3 * C)) return;
+  mask[i] = cell_changed (C, cell_epoch, since, i) ? 1 : 0;
+}
+
 // frame front end in ONE launch: blocks [0, cull_blocks) run the frustum cull of the coarse cells, the
 // rest the per-pixel pre-split.  The two are independent (the cull reads only geometry).  The work-list
 // counters and the statistics snapshot are reset by the frame-begin bookkeeping of the previous k_front launch.
@@ -285,6 +294,7 @@ __global__ void k_front (Params p, const FrameRec* __restrict__ fr, int cull_blo
         (cset ? q1 : q0)[k] = e;
       }
       if (fold) fs.visited[(size_t) cset * (n * n * n) + i] = s_fr_.seq;
+      stamp_cell (p, i, s_fr_.epoch);                   // the frame's updates, splits and prunes of this cell
     }
   }
   else
@@ -316,7 +326,7 @@ __global__ void k_front (Params p, const FrameRec* __restrict__ fr, int cull_blo
       }
       __syncwarp ();
     }
-    if (split_it) presplit_point (p, fx_, fy_, fz_);
+    if (split_it) presplit_point (p, fx_, fy_, fz_, s_fr_.epoch);
   }
   if (gated && blockIdx.x == 0 && threadIdx.x < 16)
   {
@@ -419,15 +429,19 @@ __global__ void k_edit_resolve (Params gp, const float* __restrict__ xyz, int n,
   if (m && (threadIdx.x & 31) == 0) atomicAdd (ood, (unsigned long long) __popc (m));
 }
 
-// the last point of the batch that reached each node stores its {d, w}
+// the last point of the batch that reached each node stores its {d, w}, stamps the node's cell with `epoch` and sets *wrote
 __global__ void k_edit_store (Params p, int n, const float* __restrict__ d, const float* __restrict__ w,
                               const unsigned char* __restrict__ status, const uint64_t* __restrict__ addr,
-                              uint64_t* __restrict__ keys, const int* __restrict__ last, uint32_t mask)
+                              uint64_t* __restrict__ keys, const int* __restrict__ last, uint32_t mask,
+                              unsigned long long epoch, int* __restrict__ wrote)
 {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n || status[i] != EDIT_WRITTEN) return;
   const uint64_t a = addr[i];
-  if (edit_wins (keys, last, mask, a, i)) edit_store (p, a, d[i], w[i]);
+  if (!edit_wins (keys, last, mask, a, i)) return;
+  edit_store (p, a, d[i], w[i]);
+  stamp_cell (p, edit_cell (p, a), epoch);
+  *wrote = 1;
 }
 
 // Dense crop of the box [i0, i1) x [j0, j1) x [k0, k1): one CTA per 8x8x8 tile (the finest voxels of one level L-3 node),
@@ -608,8 +622,33 @@ __device__ __forceinline__ void mc_emit (const Params& p, const McParams& mc, co
   for (int t = 0; t < ntri; ++t) okeys[tri0 + t] = k | (unsigned long long) t;
 }
 
-// marching cubes: one cube per existing leaf at or below the coarse depth
-template <bool EMIT>
+// whether a brick rooted at level R, coordinates (bx, by, bz), holds a leaf of a selected cell (McParams::cell_mask): the
+// brick's one cell when R >= C, else any of its 8^(C - R) cells.  Every lane of the warp must call it.
+__device__ __forceinline__ bool mc_brick_selected (const Params& p, const McParams& mc, int R, int bx, int by, int bz)
+{
+  if (!mc.cell_mask) return true;
+  const int d = p.C - R;
+  if (d <= 0) return mc.cell_mask[coarse_cell (p, R, bx, by, bz)] != 0;
+  if (d > 3) return false;                                      // every node of the brick lies above the coarse depth
+  bool any = false;
+  for (int c = threadIdx.x & 31; c < 1 << (3 * d); c += 32)
+  {
+    int x = bx, y = by, z = bz;
+    for (int q = d - 1; q >= 0; --q) { const int o = (c >> (3 * q)) & 7; x = (x << 1) | (o >> 2); y = (y << 1) | ((o >> 1) & 1); z = (z << 1) | (o & 1); }
+    any |= mc.cell_mask[coarse_cell (p, p.C, x, y, z)] != 0;
+  }
+  return __any_sync (0xffffffffu, any);
+}
+
+// the count pass adds a cube's triangles to its cell (McParams::cell_tris)
+__device__ __forceinline__ void mc_count_cell (const Params& p, const McParams& mc, const NodePos& n, int ntri)
+{
+  if (mc.cell_tris && ntri) atomicAdd (&mc.cell_tris[coarse_cell (p, n.level, n.x, n.y, n.z)], (unsigned long long) ntri);
+}
+
+// marching cubes: one cube per existing leaf at or below the coarse depth, in the selected cells (McParams::cell_mask).
+// CELLS = false: McParams::cell_mask and cell_tris are null, and their tests are compiled out (the full mesh).
+template <bool EMIT, bool CELLS>
 __global__ void k_mesh_bricks (Params gp, McParams mc, const int* __restrict__ list, int nbricks,
                                unsigned long long* __restrict__ total, float* __restrict__ verts, unsigned char* __restrict__ cols,
                                unsigned long long* __restrict__ okeys)
@@ -620,8 +659,9 @@ __global__ void k_mesh_bricks (Params gp, McParams mc, const int* __restrict__ l
   const int slot = list[warp];
   int t, bx, by, bz;
   brick_key_decode (p.keys[slot], t, bx, by, bz);
-  if (!brick_root_is_split (p, t, bx, by, bz)) return;         // nothing below an unsplit root exists
   const int R = tier_root_level (p, t);
+  if (CELLS && !mc_brick_selected (p, mc, R, bx, by, bz)) return;
+  if (!brick_root_is_split (p, t, bx, by, bz)) return;         // nothing below an unsplit root exists
   const uint32_t* sw = p.split + (size_t) slot * BRICK_SPLIT_WORDS;
   for (int base = 0; base < BRICK_NODES; base += 32)
   {
@@ -631,11 +671,12 @@ __global__ void k_mesh_bricks (Params gp, McParams mc, const int* __restrict__ l
     if (i < BRICK_NODES)
     {
       const BrickNode b = brick_node (p, sw, R, bx, by, bz, true, i);
-      if (b.exists && !b.split && b.level >= p.C)
+      if (b.exists && !b.split && b.level >= p.C && (!CELLS || mc_cell_selected (p, mc, b.level, b.x, b.y, b.z)))
       {
         n = brick_node_pos (p, b, slot, i);
         dw = p.nodes[(size_t) slot * BRICK_NODES + i];
         ntri = mc_leaf (p, mc, n, dw.x, dw.y, b200tsdf_mc::edge_table, b200tsdf_mc::tri_table, nullptr, nullptr);
+        if (CELLS && !EMIT) mc_count_cell (p, mc, n, ntri);
       }
     }
     unsigned long long tri0;
@@ -645,7 +686,7 @@ __global__ void k_mesh_bricks (Params gp, McParams mc, const int* __restrict__ l
 }
 
 // leaves held in the root arrays (unsplit coarse cells when Rtop == C)
-template <bool EMIT>
+template <bool EMIT, bool CELLS>
 __global__ void k_mesh_roots (Params gp, McParams mc, unsigned long long* __restrict__ total, float* __restrict__ verts, unsigned char* __restrict__ cols,
                               unsigned long long* __restrict__ okeys)
 {
@@ -657,10 +698,11 @@ __global__ void k_mesh_roots (Params gp, McParams mc, unsigned long long* __rest
   if (i < n * n * n)                                           // (the block size is a multiple of 32: every lane reaches warp_reserve)
   {
     nd = make_root (p, i / (n * n), (i / n) % n, i % n);
-    if (!is_split (p, nd))
+    if (!is_split (p, nd) && (!CELLS || mc_cell_selected (p, mc, nd.level, nd.x, nd.y, nd.z)))
     {
       dw = p.root_dw[nd.idx];
       ntri = mc_leaf (p, mc, nd, dw.x, dw.y, b200tsdf_mc::edge_table, b200tsdf_mc::tri_table, nullptr, nullptr);
+      if (CELLS && !EMIT) mc_count_cell (p, mc, nd, ntri);
     }
   }
   unsigned long long tri0;
@@ -959,6 +1001,11 @@ struct b200tsdf
   int count_set = 0;             // which of the two per-frame counter sets the last frame used
   DevBuf<int> d_culled; DevBuf<int> d_count; DevBuf<unsigned long long> d_stats;
   DevBuf<uint32_t> d_pix;        // Params::pix (grow-only)
+  // change epochs (DESIGN.md §3g): every mutation advances `epoch`; the device stamps the cells it may touch in d_cell_epoch
+  // (Params::cell_epoch, 8^C), and a change of the whole volume sets all_epoch instead.  d_cell_mask / d_cell_tris: the cell
+  // selection and per-cell triangle counts of b200tsdf_mesh_cells_device.  All three are sized by reset() (grow-only).
+  uint64_t epoch = 0, all_epoch = 0;
+  DevBuf<unsigned long long> d_cell_epoch; DevBuf<unsigned char> d_cell_mask; DevBuf<unsigned long long> d_cell_tris;
   bool timed = false;
   bool time_frames = false;      // set between profile_begin / profile_end: per-frame event records (ev_t0/ev_t1 and the ring around the dominant kernel)
   bool is_empty = true;          // TSDFVolumeOctree::is_empty_ (cpp:205, hpp:101)
@@ -1052,8 +1099,9 @@ struct b200tsdf
     q.rgb = vol.rgb; q.M = vol.M; q.ns = vol.ns; q.rgbn = vol.rgbn;
     q.root_dw = vol.root_dw; q.root_split = vol.root_split; q.root_rgb = vol.root_rgb; q.root_rgbn = vol.root_rgbn;
     q.root_M = vol.root_M; q.root_ns = vol.root_ns;
-    q.err = d_err; q.pix = d_pix; q.dbg = d_dbg;
+    q.err = d_err; q.pix = d_pix; q.dbg = d_dbg; q.cell_epoch = d_cell_epoch;
   }
+  void mark_all () { all_epoch = ++epoch; }   // a change of the whole volume: every cell counts as changed
   ~b200tsdf ();
 
   int fail (int code, const std::string& m) { err = m; return code; }
@@ -1301,8 +1349,10 @@ int b200tsdf_set_config (b200tsdf_t* h, const b200tsdf_config* cfg)
 {
   if (!h || !cfg) return B200TSDF_EINVAL;
   int dev = h->cfg_pending.device;
+  const b200tsdf_config before = h->cfg_pending;
   h->cfg_pending = *cfg;
   h->cfg_pending.device = dev;               // a handle is bound to its device at creation
+  if (std::memcmp (&before, &h->cfg_pending, sizeof (before))) h->mark_all ();
   // setGlobalTransform is the one setter that does not wait for reset () in the reference: global_transform_ is only read by
   // save () and the mesher (tsdf_volume_octree.h:131-133, cpp:242, marching_cubes_tsdf_octree.cpp:122-128)
   std::memcpy (h->cfg.global_transform, cfg->global_transform, sizeof (h->cfg.global_transform));
@@ -1388,6 +1438,9 @@ int b200tsdf_reset (b200tsdf_t* h)
       || (h->super_static && h->d_superq.grow (4096))
       || (fold && (h->d_fold.grow (fold_words (np.C)) || h->d_q1.grow ((size_t) h->Q.cap[0]))))
     return alloc_failed (h, "work queues");
+  const size_t ncells = (size_t) 1 << (3 * np.C);
+  if (h->d_cell_epoch.grow (ncells) || h->d_cell_mask.grow (ncells) || h->d_cell_tris.grow (ncells))
+    return alloc_failed (h, "cell epochs");
 
   // install the configuration
   Params& p = h->p;
@@ -1413,6 +1466,8 @@ int b200tsdf_reset (b200tsdf_t* h)
   h->fold_prev = false;
   h->half_launched = false;
   CK (cudaMemsetAsync (h->d_stats, 0, ST_TOTAL * sizeof (unsigned long long), s));
+  CK (cudaMemsetAsync (h->d_cell_epoch, 0, ncells * sizeof (unsigned long long), s));
+  h->mark_all ();
   h->kring_pending = 0; h->kring_head = 0;
   if (np.Rtop < np.C) k_insert_top_bricks<<<(unsigned) ((root_n + 127) / 128), 128, 0, s>>> (p);
   if (h->top_path && h->super_static) k_build_superq<<<(h->super_static + 127) / 128, 128, 0, s>>> (p, h->d_superq, h->super_static);
@@ -1511,6 +1566,7 @@ static void fill_rec (b200tsdf* h, FrameRec& r, const unsigned char* d_pts, size
   r.cset = h->count_set;
   r.timing = h->time_frames ? 1 : 0;
   r.seq = ++h->frame_seq;
+  r.epoch = ++h->epoch;
   const bool pub = publishes_folds (h);
   r.gated = pub && h->fold_prev;                                      // (the previous frame's kernels publish the marks it waits on)
   h->fold_prev = pub;
@@ -1526,9 +1582,9 @@ static void fill_rec (b200tsdf* h, FrameRec& r, const unsigned char* d_pts, size
 // afresh (counter set 0, no gate, fold marks cleared).
 struct FrameNumbering
 {
-  b200tsdf* h; uint32_t seq; int cset; bool fold_prev; bool enqueued = false;
-  explicit FrameNumbering (b200tsdf* h_) : h (h_), seq (h_->frame_seq), cset (h_->count_set), fold_prev (h_->fold_prev) {}
-  ~FrameNumbering () { if (!enqueued) { h->frame_seq = seq; h->count_set = cset; h->fold_prev = fold_prev; } }
+  b200tsdf* h; uint32_t seq; int cset; bool fold_prev; uint64_t epoch; bool enqueued = false;
+  explicit FrameNumbering (b200tsdf* h_) : h (h_), seq (h_->frame_seq), cset (h_->count_set), fold_prev (h_->fold_prev), epoch (h_->epoch) {}
+  ~FrameNumbering () { if (!enqueued) { h->frame_seq = seq; h->count_set = cset; h->fold_prev = fold_prev; h->epoch = epoch; } }
 };
 
 // the launches of one frame; every kernel reads the frame from *d_rec, so the launches can be captured and replayed.
@@ -2250,17 +2306,22 @@ static int edit_batch (b200tsdf* h, const float* d_xyz, size_t n, float min_size
   EditWork e = edit_work (work, n);
   unsigned char* status = d_status ? d_status : e.status;
   unsigned long long* d_ood = h->d_stats + ST_SCRATCH;
+  int* d_wrote = h->d_count + 41;
+  CK (cudaMemsetAsync (d_wrote, 0, sizeof (int), s));
   CK (cudaMemsetAsync (e.keys, 0xFF, (size_t) (e.mask + 1ull) * sizeof (uint64_t), s));
   CK (cudaMemsetAsync (e.last, 0xFF, (size_t) (e.mask + 1ull) * sizeof (int), s));
   CK (cudaMemsetAsync (d_ood, 0, sizeof (unsigned long long), s));
   const unsigned blocks = (unsigned) ((n + 127) / 128);
   k_edit_resolve<<<blocks, 128, 0, s>>> (h->p, d_xyz, (int) n, min_size, d_d, d_w, status, e.addr, e.keys, e.last, e.mask, d_ood);
-  k_edit_store<<<blocks, 128, 0, s>>> (h->p, (int) n, d_d, d_w, status, e.addr, e.keys, e.last, e.mask);
+  k_edit_store<<<blocks, 128, 0, s>>> (h->p, (int) n, d_d, d_w, status, e.addr, e.keys, e.last, e.mask, h->epoch + 1, d_wrote);
   CK (cudaGetLastError ());
   unsigned long long ood = 0;
+  int wrote = 0;
   CK (cudaMemcpyAsync (&ood, d_ood, sizeof (ood), cudaMemcpyDeviceToHost, s));
+  CK (cudaMemcpyAsync (&wrote, d_wrote, sizeof (wrote), cudaMemcpyDeviceToHost, s));
   note_device_err (h, s);
   CK (cudaStreamSynchronize (s));
+  if (wrote) ++h->epoch;                                     // the epoch the written cells were stamped with
   if (ood && h->fast_path)
   {
     h->fast_path = false; h->top_path = false;
@@ -2425,11 +2486,14 @@ int b200tsdf_render (b200tsdf_t* h, const double* pose, int downsample, void* ou
 } // extern "C"
 
 // ---- marching cubes (marching_cubes_tsdf_octree.cpp:108-236) --------------------------------------------
-// The one mesh path of b200tsdf_mesh and b200tsdf_mesh_device: the brick walk as count and emit launches, handed to
-// sort (launch), which runs them through sorted_records with the caller's destination.  A triangle is one record of 9
-// words (its three vertices) and 9 colour bytes, which is already the layout of the result.
+// The one mesh path of b200tsdf_mesh, b200tsdf_mesh_device and b200tsdf_mesh_cells_device: the brick walk as count and emit
+// launches, handed to sort (launch), which runs them through sorted_records with the caller's destination.  A triangle is one
+// record of 9 words (its three vertices) and 9 colour bytes, which is already the layout of the result.  mask (host, 8^C
+// bytes, or null for every cell) restricts the walk to the leaves of the selected coarse cells; cell_tris (host, 8^C, or null)
+// receives each cell's triangle count from the count pass.
 template <typename Sort>
-static int marching_cubes (b200tsdf* h, float w_min, int color_mode, const Sort& sort)
+static int marching_cubes (b200tsdf* h, float w_min, int color_mode, const Sort& sort, const uint8_t* mask = nullptr,
+                           unsigned long long* cell_tris = nullptr)
 {
   if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "reconstruct before reset()");
   cudaSetDevice (h->device);
@@ -2437,6 +2501,17 @@ static int marching_cubes (b200tsdf* h, float w_min, int color_mode, const Sort&
   McParams mc;
   make_mc_params (h->cfg, p, w_min, color_mode, mc);
   cudaStream_t s = h->stream;
+  const size_t ncells = (size_t) 1 << (3 * p.C);
+  if (mask)
+  {
+    CK (cudaMemcpyAsync (h->d_cell_mask, mask, ncells, cudaMemcpyHostToDevice, s));
+    mc.cell_mask = h->d_cell_mask;
+  }
+  if (cell_tris)
+  {
+    CK (cudaMemsetAsync (h->d_cell_tris, 0, ncells * sizeof (unsigned long long), s));
+    mc.cell_tris = h->d_cell_tris;
+  }
   int* list = nullptr;
   const int nb = list_bricks (h, list);
   if (nb < 0) return nb;
@@ -2444,10 +2519,19 @@ static int marching_cubes (b200tsdf* h, float w_min, int color_mode, const Sort&
   auto launch = [&] (auto emit, unsigned long long* total, unsigned long long* keys, void* v, unsigned char* c)
   {
     constexpr bool E = decltype (emit)::value;
-    if (nb) k_mesh_bricks<E><<<bgrid, 128, 0, s>>> (p, mc, list, nb, total, (float*) v, c, keys);
-    k_mesh_roots<E><<<rgrid, 128, 0, s>>> (p, mc, total, (float*) v, c, keys);
+    if (mask || cell_tris)
+    {
+      if (nb) k_mesh_bricks<E, true><<<bgrid, 128, 0, s>>> (p, mc, list, nb, total, (float*) v, c, keys);
+      k_mesh_roots<E, true><<<rgrid, 128, 0, s>>> (p, mc, total, (float*) v, c, keys);
+    }
+    else
+    {
+      if (nb) k_mesh_bricks<E, false><<<bgrid, 128, 0, s>>> (p, mc, list, nb, total, (float*) v, c, keys);
+      k_mesh_roots<E, false><<<rgrid, 128, 0, s>>> (p, mc, total, (float*) v, c, keys);
+    }
   };
   if (int rc = sort (launch)) return rc;
+  if (cell_tris) CK (cudaMemcpyAsync (cell_tris, h->d_cell_tris, ncells * sizeof (unsigned long long), cudaMemcpyDeviceToHost, s));
   return check_device_err (h);
 }
 
@@ -2471,9 +2555,17 @@ int b200tsdf_mesh (b200tsdf_t* h, float w_min, int color_mode, float** verts, ui
 int b200tsdf_mesh_device (b200tsdf_t* h, float w_min, int color_mode, float* d_verts, uint8_t* d_rgb, size_t capacity,
                           size_t* nverts)
 {
+  return b200tsdf_mesh_cells_device (h, w_min, color_mode, nullptr, d_verts, d_rgb, capacity, nverts, nullptr);
+}
+
+int b200tsdf_mesh_cells_device (b200tsdf_t* h, float w_min, int color_mode, const uint8_t* mask, float* d_verts, uint8_t* d_rgb,
+                                size_t capacity, size_t* nverts, int64_t* cell_nverts)
+{
   if (!h || !nverts) return B200TSDF_EINVAL;
   *nverts = 0;
   if ((uintptr_t) d_verts & 3) return h->fail (B200TSDF_EINVAL, "d_verts must be 4-byte aligned");
+  if ((mask || cell_nverts) && h->has_volume && h->p.shard_count > 1)
+    return h->fail (B200TSDF_ESTATE, "mesh of selected cells on a shard: mesh the replica built by b200tsdf_gather_volume");
   unsigned long long ntri = 0;
   auto dest = [&] (unsigned long long n, void*& v_out, unsigned char*& c_out)
   {
@@ -2485,7 +2577,35 @@ int b200tsdf_mesh_device (b200tsdf_t* h, float w_min, int color_mode, float* d_v
     return (int) B200TSDF_OK;
   };
   auto sort = [&] (const auto& launch) { return sorted_records (h, "triangles", 9, 3 * h->p.L + 3, launch, dest, ntri); };
-  return marching_cubes (h, w_min, color_mode, sort);
+  // the per-cell triangle counts land in cell_nverts itself, then become vertex counts
+  static_assert (sizeof (int64_t) == sizeof (unsigned long long), "cell_nverts holds the device's 64-bit counts");
+  if (int rc = marching_cubes (h, w_min, color_mode, sort, mask, reinterpret_cast<unsigned long long*> (cell_nverts))) return rc;
+  if (cell_nverts)
+    for (size_t c = 0, n = (size_t) 1 << (3 * h->p.C); c < n; ++c) cell_nverts[c] *= 3;
+  return B200TSDF_OK;
+}
+
+int b200tsdf_changed_cells (b200tsdf_t* h, uint64_t since, uint64_t* now, uint8_t* mask)
+{
+  if (!h || !now) return B200TSDF_EINVAL;
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "changed_cells before reset()");
+  if (h->p.shard_count > 1)
+    return h->fail (B200TSDF_ESTATE, "changed_cells on a shard: shards keep no change epochs; mesh the replica built by b200tsdf_gather_volume");
+  cudaSetDevice (h->device);
+  cudaStream_t s = h->stream;
+  const int n = 1 << h->p.C;
+  const size_t ncells = (size_t) n * n * n;
+  if (mask && !(since == 0 || h->all_epoch > since))
+  {
+    k_changed_cells<<<(unsigned) ((ncells + 255) / 256), 256, 0, s>>> (h->p.C, h->d_cell_epoch, (unsigned long long) since, h->d_cell_mask);
+    CK (cudaGetLastError ());
+    CK (cudaMemcpyAsync (mask, h->d_cell_mask, ncells, cudaMemcpyDeviceToHost, s));
+  }
+  if (int rc = check_device_err (h)) return rc;              // (waits for the handle's stream)
+  if (int rc = pending_device_err (h)) return rc;
+  if (mask && (since == 0 || h->all_epoch > since)) std::memset (mask, 1, ncells);
+  *now = h->epoch;
+  return B200TSDF_OK;
 }
 
 } // extern "C"
@@ -3282,6 +3402,7 @@ int load_device_body (b200tsdf* h, const unsigned char* d_body, size_t len, bool
 // after a body is in: isEmpty from the header, the fast route only for values fusion produces, and the device error bits
 int load_finish (b200tsdf* h, int is_empty, unsigned long long ood, bool on_device)
 {
+  h->mark_all ();
   h->is_empty = is_empty != 0;
   h->loaded_on_device = on_device;
   if (ood && h->fast_path)
@@ -3518,6 +3639,7 @@ int b200tsdf_import_shard (b200tsdf_t* h, const void* buf, size_t nbytes)
   cudaSetDevice (h->device);
   int rc = b200tsdf_sync (h);
   if (rc) return rc;
+  h->mark_all ();                                          // (before the first write: a failure below may leave part of it)
   const unsigned char* o = (const unsigned char*) buf + sizeof (ShardHeader);
   size_t nr = hd.n_roots, nb = hd.n_bricks;
   std::vector<int> ridx (nr); std::vector<float2> rdw (nr); std::vector<unsigned char> rsp (nr); std::vector<uchar4> rrgb (nr); std::vector<float> rM (nr); std::vector<int> rns (nr);

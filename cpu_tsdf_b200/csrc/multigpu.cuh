@@ -375,6 +375,7 @@ int b200tsdf_gather_volume (b200tsdf_t* h, b200tsdf_t* full, int root)
   else
   {
     const Params& fp = full->p;
+    full->mark_all ();                                     // (before the first write: a failure below may leave part of it)
     // own shard: same device, straight from this handle's arrays
     k_merge_roots<<<(unsigned) ((rn + 127) / 128), 128, 0, s>>> (fp, (int) rn, rk, nr, p.root_dw, p.root_split, p.root_rgb);
     if (nb) k_load_bricks<<<nb, 128, 0, s>>> (fp, g_keys, nb, g_nodes, g_split, g_rgb, nullptr, nullptr);

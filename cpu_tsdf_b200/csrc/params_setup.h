@@ -127,6 +127,7 @@ inline void make_mc_params (const b200tsdf_config& c, const Params& p, float w_m
   float lo = voxel_center1 (p, 0), hi = voxel_center1 (p, p.res);
   for (int k = 0; k < 3; ++k) { mc.lower[k] = lo; mc.size_voxel[k] = (hi - lo) * (1.0f / (float) p.res); }
   for (int i = 0; i < 12; ++i) mc.gt[i] = c.global_transform[i];
+  mc.cell_mask = nullptr; mc.cell_tris = nullptr;
 }
 
 } // namespace b2

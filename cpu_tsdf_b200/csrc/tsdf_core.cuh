@@ -166,6 +166,8 @@ struct Params
   unsigned long long* dbg;    // optional phase timing of k_celltop_up (b200tsdf_debug_timing), normally null
   uint32_t* pix;              // [2][width * height] pixel planes (frame_plane), written by k_front: {z bits, bgra} per pixel
                               // with colour, z bits alone without (read by the fast observation, obs_fast.cuh)
+  unsigned long long* cell_epoch;  // [8^C] per coarse cell, the epoch of the last mutation that may have touched it
+                                   // (b200tsdf_changed_cells, DESIGN.md §3g), or null: nothing is stamped
 };
 
 struct Frame
@@ -850,15 +852,31 @@ B2_HD bool owns_cell (const Params& p, int cx, int cy, int cz)
   return (int) (h % (uint32_t) p.shard_count) == p.shard_rank;
 }
 
-B2_HD void presplit_point (const Params& p, int fx_, int fy_, int fz_)
+// the coarse cell ((x n + y) n + z, n = 2^C; the layout of b200tsdf_frustum_cull's mask) of node (x, y, z) at level >= C
+B2_HD int coarse_cell (const Params& p, int level, int x, int y, int z)
 {
+  const int sh = level - p.C, n = 1 << p.C;
+  return ((x >> sh) * n + (y >> sh)) * n + (z >> sh);
+}
+// a mutation at `epoch` may have changed the nodes of coarse cell c
+B2_HD void stamp_cell (const Params& p, int c, unsigned long long epoch)
+{
+  if (p.cell_epoch) p.cell_epoch[c] = epoch;
+}
+
+// A split bit this call sets, that was not set, removes a leaf and so its triangles: its cell is stamped with `epoch`, whether
+// or not the frame culls that cell in (a point beyond max_sensor_dist still splits its cell).  Nothing is stamped when
+// Params::cell_epoch is null, as in the callers that keep no epochs.
+B2_HD void presplit_point (const Params& p, int fx_, int fy_, int fz_, unsigned long long epoch = 0)
+{
+  const int cell = coarse_cell (p, p.L, fx_, fy_, fz_);
   // root array node (level Rtop) if it is a coarse-or-deeper level
   if (p.Rtop >= p.C)
   {
     int sh = p.L - p.Rtop;
     int ri = root_index (p, fx_ >> sh, fy_ >> sh, fz_ >> sh);
     uint32_t m = 1u << (ri & 31);
-    if (!(p.root_split[ri >> 5] & m)) atomic_or32 (&p.root_split[ri >> 5], m);
+    if (!(p.root_split[ri >> 5] & m) && !(atomic_or32 (&p.root_split[ri >> 5], m) & m)) stamp_cell (p, cell, epoch);
   }
   for (int t = p.T - 1; t >= 0; --t)
   {
@@ -875,7 +893,7 @@ B2_HD void presplit_point (const Params& p, int fx_, int fy_, int fz_)
       int j = path_index (k, fx_ >> s2, fy_ >> s2, fz_ >> s2);
       uint32_t m = 1u << (j & 31);
       uint32_t* w = sw + split_word_base (k) + (j >> 5);
-      if (!(*w & m)) atomic_or32 (w, m);
+      if (!(*w & m) && !(atomic_or32 (w, m) & m)) stamp_cell (p, cell, epoch);
     }
   }
 }
@@ -1052,6 +1070,23 @@ B2_HD bool edit_wins (uint64_t* keys, const int* last, uint32_t mask, uint64_t a
 B2_HD void edit_store (const Params& p, uint64_t addr, float d, float w)
 {
   *node_dw (p, edit_node (addr)) = make_float2 (d, w);
+}
+
+// the coarse cell of the node at a storage address (written nodes lie at or below the coarse depth, see edit_resolve)
+B2_HD int edit_cell (const Params& p, uint64_t addr)
+{
+  const NodePos n = edit_node (addr);
+  if (n.slot < 0)
+  {
+    const int r = 1 << p.Rtop;
+    return coarse_cell (p, p.Rtop, n.idx / (r * r), (n.idx / r) % r, n.idx % r);
+  }
+  int t, bx, by, bz;
+  brick_key_decode (p.keys[n.slot], t, bx, by, bz);
+  const int k = n.idx < 8 ? 1 : (n.idx < 72 ? 2 : 3), j = n.idx - node_offset (k);
+  int x = bx, y = by, z = bz;
+  for (int q = k - 1; q >= 0; --q) { const int c = (j >> (3 * q)) & 7; x = (x << 1) | (c >> 2); y = (y << 1) | ((c >> 1) & 1); z = (z << 1) | (c & 1); }
+  return coarse_cell (p, tier_root_level (p, t) + k, x, y, z);
 }
 
 // ---- dense crop: the point lookup at every voxel centre of a box, one 8x8x8 tile at a time -------------------------------
@@ -1355,7 +1390,30 @@ struct McParams
   int color_mode;               // 0 none, 1 rgb, 2 confidence
   float lower[3], size_voxel[3];// pcl::MarchingCubes lower_boundary_, size_voxel_ (set by setInputTSDF, cpp:43-83)
   double gt[12];                // global transform rows 0..2
+  const unsigned char* cell_mask;  // [8^C]: mesh only the leaves of coarse cells c with cell_mask[c] != 0; null: every cell
+  unsigned long long* cell_tris;   // [8^C]: the count pass adds each cell's triangles here; null: no per-cell counts
 };
+
+// b200tsdf_changed_cells: whether a mesh of cell i taken at epoch `since` may differ from one taken now, i.e. whether some cell
+// i + {0,1}^3 inside the grid was stamped after `since` (a cube reads the nodes at voxel idx + {0,1}^3, mc_leaf)
+B2_HD bool cell_changed (int C, const unsigned long long* cell_epoch, unsigned long long since, int i)
+{
+  const int n = 1 << C;
+  const int z = i % n, y = (i / n) % n, x = i / (n * n);
+  bool changed = false;
+  for (int d = 0; d < 8; ++d)
+  {
+    const int a = x + (d >> 2), b = y + ((d >> 1) & 1), c = z + (d & 1);
+    if (a < n && b < n && c < n) changed |= cell_epoch[((size_t) a * n + b) * n + c] > since;
+  }
+  return changed;
+}
+
+// whether the leaf (level, x, y, z), level >= C, is in a selected cell
+B2_HD bool mc_cell_selected (const Params& p, const McParams& mc, int level, int x, int y, int z)
+{
+  return !mc.cell_mask || mc.cell_mask[coarse_cell (p, level, x, y, z)] != 0;
+}
 
 // Position of a leaf in the reference's mesh order.  performReconstruction walks the octree depth first with the
 // children in index order (octree.cpp:257-264: x is the high bit, then y, then z), one cube per leaf, so leaves come

@@ -225,6 +225,27 @@ void b200tsdf_free (void* p);
 int  b200tsdf_mesh_device (b200tsdf_t* h, float w_min, int color_mode, float* d_verts, uint8_t* d_rgb, size_t capacity,
                            size_t* nverts);
 
+/* ---- incremental meshing: change epochs per coarse cell (DESIGN.md §3g) ------------------------------------
+ * A handle keeps a 64-bit epoch, 0 at create.  Every integrated frame (every route), every node-writing
+ * b200tsdf_set_containing_voxels[_device] call and every whole-volume change (reset, load, load_device, import_shard, the full
+ * handle of gather_volume, a set_config that changes a field) advances it by one.  resize_pool, saves, reads and refused calls
+ * do not.  The mesh triangles of coarse cell c depend only on the nodes of cells c + {0,1}^3, and the full mesh is the runs of
+ * the cells one after the other in Morton order, so the triangles of the cells a change may have touched can be re-meshed and
+ * spliced into an earlier mesh.
+ *
+ * *now = the handle's epoch.  mask (optional, 8^C bytes, host, layout of b200tsdf_frustum_cull): mask[c] = 1 iff a mesh of
+ * cell c taken at epoch `since` may differ from one taken now, i.e. some cell c + {0,1}^3 was stamped after `since`
+ * (since = 0: every cell).  Ordered after all queued work (waits for the handle's stream).  B200TSDF_ESTATE before reset()
+ * and on a sharded handle; a latched device error is reported as by the other reads. */
+int  b200tsdf_changed_cells (b200tsdf_t* h, uint64_t since, uint64_t* now, uint8_t* mask);
+/* b200tsdf_mesh_device restricted to the leaves whose coarse cell has mask[c] != 0 (mask == NULL: every cell): exactly the
+ * triangles of the full mesh that lie in those cells, in the same relative order, so a cell's triangles are contiguous and
+ * cells follow in Morton order.  cell_nverts (optional, host, 8^C int64): the vertex count of each cell, 0 where not selected.
+ * d_verts == NULL counts only (cell_nverts is filled); capacity, alignment, colour and error rules as b200tsdf_mesh_device.
+ * With a mask or cell_nverts, B200TSDF_ESTATE on a sharded handle. */
+int  b200tsdf_mesh_cells_device (b200tsdf_t* h, float w_min, int color_mode, const uint8_t* mask,
+                                 float* d_verts, uint8_t* d_rgb, size_t capacity, size_t* nverts, int64_t* cell_nverts);
+
 /* ---- mesh post-processing of the reference's `integrate` program (no volume handle needed) ----------
  * Meshes are indexed: nverts xyz triples + ntris index triples (a marching-cubes soup is tris = 0,1,2,...).
  * Outputs are malloc'ed by the library; release each with b200tsdf_mesh_free.  Vertex colours are not

@@ -303,6 +303,21 @@ public:
     return status_ == 0;
   }
 
+  // extension: change epochs per coarse cell (b200tsdf_changed_cells).  *now receives the volume's epoch; mask, when given, is
+  // resized to 8^C and set to 1 for every cell whose mesh may differ from one taken at epoch `since`.  Sets status ().
+  bool changedCells (std::uint64_t since, std::uint64_t* now, std::vector<std::uint8_t>* mask = nullptr) const
+  {
+    if (!h_) { status_ = B200TSDF_ENODEVICE; return false; }
+    if (mask)
+    {
+      b200tsdf_stats st;
+      if ((status_ = b200tsdf_get_stats (h_, &st)) != 0) return false;
+      mask->assign (static_cast<std::size_t> (1) << (3 * st.coarse_level), 0);
+    }
+    status_ = b200tsdf_changed_cells (h_, since, now, mask ? mask->data () : nullptr);
+    return status_ == 0;
+  }
+
   PointXYZ getVoxelCenter (std::size_t x, std::size_t y, std::size_t z) const                      // cpp:553-560
   { float o[3] = { 0, 0, 0 }; b200tsdf_voxel_center (h_, (std::int64_t) x, (std::int64_t) y, (std::int64_t) z, o); PointXYZ p; p.x = o[0]; p.y = o[1]; p.z = o[2]; return p; }
   bool getVoxelIndex (float x, float y, float z, int& x_i, int& y_i, int& z_i) const               // cpp:562-574
@@ -497,6 +512,24 @@ public:
     return true;
   }
 #endif
+
+  // extension: the mesh of the coarse cells with mask[c] != 0 (mask: 8^C bytes from changedCells, or nullptr for every cell)
+  // into device memory (b200tsdf_mesh_cells_device): the full mesh's triangles of those cells, in the same order.
+  // cell_nverts, when given, is resized to 8^C and receives each cell's vertex count.  Returns a B200TSDF_ code.
+  int reconstructCellsDevice (const std::uint8_t* mask, float* d_verts, std::uint8_t* d_rgb, std::size_t capacity, std::size_t* nverts,
+                              std::vector<std::int64_t>* cell_nverts = nullptr) const
+  {
+    if (!tsdf_volume_ || !tsdf_volume_->handle ()) return B200TSDF_ENODEVICE;
+    int mode = color_by_confidence_ ? 2 : (color_by_rgb_ ? 1 : 0);
+    if (cell_nverts)
+    {
+      b200tsdf_stats st;
+      if (int rc = b200tsdf_get_stats (tsdf_volume_->handle (), &st)) return rc;
+      cell_nverts->assign (static_cast<std::size_t> (1) << (3 * st.coarse_level), 0);
+    }
+    return b200tsdf_mesh_cells_device (tsdf_volume_->handle (), w_min_, mode, mask, d_verts, d_rgb, capacity, nverts,
+                                       cell_nverts ? cell_nverts->data () : nullptr);
+  }
 
 private:
   TSDFVolumeOctree::ConstPtr tsdf_volume_;
