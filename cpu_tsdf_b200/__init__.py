@@ -83,7 +83,12 @@ EXPORTS = [
     "b200tsdf_containing_voxels", "b200tsdf_containing_voxels_device", "b200tsdf_dense_device",
     "b200tsdf_set_containing_voxels", "b200tsdf_set_containing_voxels_device",
     "b200tsdf_changed_cells", "b200tsdf_mesh_cells_device",
+    "b200tsdf_integrate_depth", "b200tsdf_integrate_depth_batch_device", "b200tsdf_depth_to_cloud_device",
 ]
+
+# depth formats of the depth-image entry points (B200TSDF_DEPTH_*)
+DEPTH_U16 = 1
+DEPTH_F32 = 2
 
 # b200tsdf_voxel (include/b200tsdf.h): one record of getContainingVoxel; level -1 = NULL
 VOXEL_DTYPE = np.dtype([("level", "<i4"), ("x", "<i4"), ("y", "<i4"), ("z", "<i4"),
@@ -139,6 +144,9 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_integrate_unorganized.argtypes = [vp, vp, C.c_size_t, C.c_size_t, C.c_int, C.c_int, C.POINTER(OrganizeOpts), vp]
     lib.b200tsdf_integrate_unorganized_batch_device.argtypes = [vp, C.c_int, vp, C.POINTER(C.c_size_t), C.c_size_t, C.c_int, C.c_int,
                                                                 C.POINTER(OrganizeOpts), vp]
+    lib.b200tsdf_integrate_depth.argtypes = [vp, vp, C.c_int, C.c_float, vp, C.c_int, C.c_int, vp]
+    lib.b200tsdf_integrate_depth_batch_device.argtypes = [vp, C.c_int, vp, C.c_int, C.c_float, vp, C.c_int, C.c_int, vp]
+    lib.b200tsdf_depth_to_cloud_device.argtypes = [vp, vp, C.c_int, C.c_float, vp, C.c_int, C.c_int, vp]
     lib.b200tsdf_query.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.b200tsdf_interpolate.argtypes = [vp, vp, C.c_int, vp, vp]
     lib.b200tsdf_render.argtypes = [vp, vp, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, vp]
@@ -180,6 +188,41 @@ def load_library() -> C.CDLL:
 
 def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def depth_to_cloud(depth, intrinsics, rgb=None, depth_scale=1e-3) -> np.ndarray:
+    """The organised cloud of a depth frame, as integrateDepth fuses it: [H, W, 8] float32 in integrateCloud's 32-byte
+    pcl::PointXYZRGBA layout (x, y, z, 1.0, colour bytes b, g, r, 255, three zero floats).
+
+    depth: [H, W] uint16 (sensor units) or float32; intrinsics: (fx, fy, cx, cy) of the volume, used rounded to float;
+    rgb: None or [H, W, 3] uint8 R, G, B.  For pixel (u, v), every operation float32 and rounded to nearest:
+    z = D * depth_scale, x = (u - cx) * z / fx, y = (v - cy) * z / fy; a pixel with D == 0 or z not finite is
+    x = y = z = NaN.  Without rgb the colour bytes are 0, 0, 0, 255 (the default point)."""
+    d = np.asarray(depth)
+    if d.ndim != 2 or d.dtype not in (np.uint16, np.float32):
+        raise ValueError("depth must be an [H, W] uint16 or float32 array")
+    H, W = d.shape
+    fx, fy, cx, cy = (np.float32(v) for v in intrinsics)
+    out = np.zeros((H, W, 8), np.float32)
+    with np.errstate(all="ignore"):
+        z = d.astype(np.float32) * np.float32(depth_scale)
+        u = np.arange(W, dtype=np.float32)[None, :]
+        v = np.arange(H, dtype=np.float32)[:, None]
+        x = ((u - cx) * z) / fx
+        y = ((v - cy) * z) / fy
+    bad = (d == 0) | ~np.isfinite(z)
+    out[..., 0] = np.where(bad, np.float32(np.nan), x)
+    out[..., 1] = np.where(bad, np.float32(np.nan), y)
+    out[..., 2] = np.where(bad, np.float32(np.nan), z)
+    out[..., 3] = 1.0
+    col = out.view(np.uint8).reshape(H, W, 32)
+    col[..., 19] = 255
+    if rgb is not None:
+        c = np.asarray(rgb, dtype=np.uint8)
+        if c.shape != (H, W, 3):
+            raise ValueError("rgb must be [H, W, 3] uint8 with the depth map's size")
+        col[..., 16], col[..., 17], col[..., 18] = c[..., 2], c[..., 1], c[..., 0]
+    return out
 
 
 def _pose(trans) -> np.ndarray:
@@ -427,6 +470,56 @@ class TSDFVolumeOctree:
         opts = OrganizeOpts(float(cloud_units), int(bool(zero_nans)), None if tf is None else tf.ctypes.data)
         self._check(self._lib.b200tsdf_integrate_unorganized_batch_device(self._h, n, arr, cnt, stride, 0, rgba_off, C.byref(opts), _ptr(ps)))
         return True
+
+    def integrateDepth(self, depth: np.ndarray, trans=np.eye(4), rgb=None, depth_scale=1e-3) -> bool:
+        """One depth frame from host memory: exactly integrateCloud(depth_to_cloud(depth, intrinsics, rgb, depth_scale)),
+        with the depth map ([H, W] uint16 or float32, the configured image size) and the registered colour ([H, W, 3] uint8
+        R, G, B, or None) unprojected on the device.  The arrays may be reused when the call returns."""
+        d = np.ascontiguousarray(depth)
+        if d.dtype == np.uint16:
+            fmt = DEPTH_U16
+        elif d.dtype == np.float32:
+            fmt = DEPTH_F32
+        else:
+            raise ValueError("depth must be uint16 or float32")
+        if d.ndim != 2:
+            raise ValueError("depth must be [H, W]")
+        c = None
+        if rgb is not None:
+            c = np.ascontiguousarray(rgb, dtype=np.uint8)
+            if c.shape != d.shape + (3,):
+                raise ValueError("rgb must be [H, W, 3] uint8 with the depth map's size")
+        pose = _pose(trans)
+        self._check(self._lib.b200tsdf_integrate_depth(self._h, _ptr(d), fmt, float(depth_scale), _ptr(c), d.shape[1], d.shape[0], _ptr(pose)))
+        return True
+
+    def integrateDepthBatchDevice(self, d_depth_ptrs, poses, *, depth_format: int, depth_scale: float, d_rgb_ptrs=None,
+                                  width: int | None = None, height: int | None = None) -> bool:
+        """len(d_depth_ptrs) consecutive integrateDepth calls on depth maps resident in device memory (integer device pointers,
+        DEPTH_U16 or DEPTH_F32, the configured image size unless width / height say otherwise), with optional device colour
+        images (d_rgb_ptrs: None or one pointer per frame).  One record upload and one graph launch per 32 frames.
+        Asynchronous."""
+        n = len(d_depth_ptrs)
+        if len(poses) != n or (d_rgb_ptrs is not None and len(d_rgb_ptrs) != n):
+            raise ValueError("one pose (and colour image) per depth map")
+        W = self._cfg.image_width if width is None else width
+        H = self._cfg.image_height if height is None else height
+        arr = (C.c_void_p * max(n, 1))(*[C.c_void_p(int(x) if x else None) for x in d_depth_ptrs])
+        rgb = None if d_rgb_ptrs is None else (C.c_void_p * max(n, 1))(*[C.c_void_p(int(x) if x else None) for x in d_rgb_ptrs])
+        ps = np.ascontiguousarray(np.stack([_pose(t) for t in poses]) if n else np.zeros((0, 4, 4)), dtype=np.float64)
+        self._check(self._lib.b200tsdf_integrate_depth_batch_device(self._h, n, arr, int(depth_format), float(depth_scale), rgb,
+                                                                    W, H, _ptr(ps)))
+        return True
+
+    def depthToCloudDevice(self, d_depth, d_out, *, depth_format: int, depth_scale: float, d_rgb=None,
+                           width: int | None = None, height: int | None = None):
+        """The organised cloud of one device depth map written to d_out (device, 16-byte aligned) as 16-byte pixels
+        {x, y, z, colour bytes b, g, r, a}: depth_to_cloud's floats 0-2 and 4.  Returns when written."""
+        W = self._cfg.image_width if width is None else width
+        H = self._cfg.image_height if height is None else height
+        dp = lambda x: C.c_void_p(int(x)) if x else None
+        self._check(self._lib.b200tsdf_depth_to_cloud_device(self._h, dp(d_depth), int(depth_format), float(depth_scale), dp(d_rgb),
+                                                             W, H, dp(d_out)))
 
     def _query(self, pts, what, mode):
         xyz = np.ascontiguousarray(pts, dtype=np.float32).reshape(-1, 3)

@@ -10,6 +10,7 @@
 #include "brick_kernels.cuh"
 #include "brick_direct.cuh"
 #include "organize.cuh"
+#include "depth.cuh"
 #include "mesh_sort.h"
 #include "host_pack.h"
 #include "vol_io.cuh"
@@ -128,6 +129,12 @@ constexpr size_t ORG_HDR = (sizeof (OrgBatch) + 15) & ~(size_t) 15;
 constexpr int BRING_SPAN = FRAME_RING / 2 + (int) ((ORG_HDR + ORG_MAX_FRAMES * sizeof (OrgRec) + sizeof (FrameRec) - 1) / sizeof (FrameRec));
 OrgBatch* org_block (FrameRec* recs, int m) { return reinterpret_cast<OrgBatch*> (recs + m); }
 OrgRec* org_recs (FrameRec* recs, int m) { return reinterpret_cast<OrgRec*> (reinterpret_cast<unsigned char*> (recs + m) + ORG_HDR); }
+// a batch of depth frames has its depth block (DepthBatch) in the same place
+static_assert (sizeof (DepthBatch) <= ORG_HDR + ORG_MAX_FRAMES * sizeof (OrgRec), "a depth block fits where the organise block goes");
+DepthBatch* depth_block (FrameRec* recs, int m) { return reinterpret_cast<DepthBatch*> (recs + m); }
+// what comes in front of the frames of a batch: nothing (organised clouds), the organise launches, or the depth unprojection
+enum FrontEnd { FRONT_NONE, FRONT_ORGANIZE, FRONT_DEPTH };
+constexpr int DEPTH_SLOTS = 3;  // pinned staging slots (and device raw buffers) of b200tsdf_integrate_depth
 
 // ---------------------------------------------------------------------------------------------
 // kernels
@@ -1042,9 +1049,16 @@ struct b200tsdf
   Event ev_half_done[2]; bool half_used[2] = { false, false };
   cudaGraphExec_t batch_exec[2][FRAME_RING / 2 + 1] = {};
   cudaGraphExec_t unorg_exec[2][FRAME_RING / 2 + 1] = {};   // the same with the three organise launches in front
+  cudaGraphExec_t depth_exec[2][FRAME_RING / 2 + 1] = {};   // the same with the depth unprojection in front
   // unorganised batches: the keys, filled counters and 16-byte organised images of one record half (organise and fuse of both
   // halves run on `stream`, so one set serves both); allocated at the first unorganised integrate, freed by reset()
   DevBuf<unsigned char> d_org;
+  // depth frames from host memory (b200tsdf_integrate_depth): the caller's depth and colour are copied into one of
+  // DEPTH_SLOTS pinned slots, uploaded on copy_stream into that slot's device buffer and unprojected from there.  A slot is
+  // rewritten once its upload has run (ev_dcopied), its device buffer once the unprojection that read it has (ev_dconsumed).
+  Staging h_depth[DEPTH_SLOTS]; DevBuf<unsigned char> d_depth_raw[DEPTH_SLOTS];
+  Event ev_dcopied[DEPTH_SLOTS], ev_dconsumed[DEPTH_SLOTS];
+  uint64_t depth_no = 0;
   // multi-GPU (multigpu.cuh): NCCL communicator (opaque here), row-sliced uploads
   void* comm = nullptr; int comm_rank = 0, comm_size = 1;
   DevBuf<unsigned char> d_rows_raw[2], d_rows_full[2];
@@ -1131,6 +1145,7 @@ void drop_batch_graphs (b200tsdf* h)
     {
       if (h->batch_exec[a][n]) { cudaGraphExecDestroy (h->batch_exec[a][n]); h->batch_exec[a][n] = nullptr; }
       if (h->unorg_exec[a][n]) { cudaGraphExecDestroy (h->unorg_exec[a][n]); h->unorg_exec[a][n] = nullptr; }
+      if (h->depth_exec[a][n]) { cudaGraphExecDestroy (h->depth_exec[a][n]); h->depth_exec[a][n] = nullptr; }
     }
 }
 
@@ -1319,6 +1334,7 @@ int b200tsdf_create (const b200tsdf_config* cfg, b200tsdf_t** out)
          && !h->h_rrec.alloc ((size_t) RENDER_SEGS * RENDER_CHUNK)
          && create_events (h->ev_ring, 2, nt) && create_events (h->ev_rows_done, 2, nt) && create_events (h->ev_bring, BATCH_SEGS, nt)
          && create_events (h->ev_half_done, 2, nt) && create_events (h->ev_copied, 2, nt) && create_events (h->ev_consumed, 2, nt)
+         && create_events (h->ev_dcopied, DEPTH_SLOTS, nt) && create_events (h->ev_dconsumed, DEPTH_SLOTS, nt)
          && create_events (h->ev_rrec, RENDER_SEGS, nt) && create_events (&h->ev_rows_ready[0][0], 64, nt) && create_events (&h->ev_rows_up[0][0], 64, nt)
          && create_events (&h->ev_t0, 1, cudaEventDefault) && create_events (&h->ev_t1, 1, cudaEventDefault)
          && create_events (&h->ev_p0, 1, cudaEventDefault) && create_events (&h->ev_p1, 1, cudaEventDefault)
@@ -1737,10 +1753,12 @@ int b200tsdf_integrate_device (b200tsdf_t* h, const void* d_points, size_t strid
 // into one half of the device slots; (2) the captured launches of that half are replayed on the compute stream.  The row
 // path (multigpu.cuh) uploads the records on its copy stream AHEAD of the frames themselves — a record upload issued on
 // the compute stream would queue behind every frame copy already submitted to the one host-to-device copy engine.
-// ob / orecs: the organise block of an unorganised batch, which travels in the same copy behind the frame records
+// ob / orecs: the organise block of an unorganised batch, db: the depth block of a depth batch; either travels in the same
+// copy behind the frame records
 // The caller has checked every argument (d_points[i] are not null) and holds a FrameNumbering until batch_launch has returned.
 static int batch_records (b200tsdf* h, int m, const void* const* d_points, size_t stride, int xyz_off, int rgba_off, int width, int height,
-                          const double* poses_c2w, cudaStream_t rec_stream, const OrgBatch* ob = nullptr, const OrgRec* orecs = nullptr)
+                          const double* poses_c2w, cudaStream_t rec_stream, const OrgBatch* ob = nullptr, const OrgRec* orecs = nullptr,
+                          const DepthBatch* db = nullptr)
 {
   const int a = h->bring_half, sg = h->bring_seg;
   if (h->bring_used[sg]) CK (cudaEventSynchronize (h->ev_bring[sg]));    // the copy that last read this staging segment has run
@@ -1753,6 +1771,11 @@ static int batch_records (b200tsdf* h, int m, const void* const* d_points, size_
     *org_block (recs, m) = *ob;
     std::memcpy (org_recs (recs, m), orecs, (size_t) m * sizeof (OrgRec));
     bytes += ORG_HDR + (size_t) m * sizeof (OrgRec);
+  }
+  else if (db)
+  {
+    *depth_block (recs, m) = *db;
+    bytes += sizeof (DepthBatch);
   }
   // the device half is rewritten only after the launches that last read it (other stream: wait for their event)
   if (rec_stream != h->stream && h->half_used[a]) CK (cudaStreamWaitEvent (rec_stream, h->ev_half_done[a], 0));
@@ -1786,25 +1809,39 @@ static int launch_organize (b200tsdf* h, cudaStream_t s, const OrgBatch* d_ob, c
   return B200TSDF_OK;
 }
 
-// organize: the records carry the organise block of an unorganised batch (batch_records), whose three launches come first
-static int batch_launch (b200tsdf* h, int m, bool organize = false)
+// the unprojection of m depth frames (depth.cuh) into m images of 16-byte pixels
+static int launch_depth (b200tsdf* h, cudaStream_t s, const DepthBatch* d_db, int m, unsigned char* out)
+{
+  const int npix = (int) org_npix (h);
+  k_depth_unproject<<<dim3 ((npix + 255) / 256, m), 256, 0, s>>> (d_db, npix, out);
+  h->launches += 1;
+  CK (cudaGetLastError ());
+  return B200TSDF_OK;
+}
+
+// front: FRONT_ORGANIZE, the records carry the organise block of an unorganised batch (batch_records), whose three launches
+// come first; FRONT_DEPTH, they carry the depth block of a depth batch, whose unprojection comes first
+static int batch_launch (b200tsdf* h, int m, FrontEnd front = FRONT_NONE)
 {
   cudaStream_t s = h->stream;
   const int a = h->bring_half;
   FrameRec* const d_recs = h->d_bring + a * BRING_SPAN;
-  cudaGraphExec_t& exec = (organize ? h->unorg_exec : h->batch_exec)[a][m];   // (nothing of a frame is baked into the launches: they read the record)
-  const int org_launches = organize ? 3 : 0;
+  // (nothing of a frame is baked into the launches: they read the record)
+  cudaGraphExec_t& exec = (front == FRONT_ORGANIZE ? h->unorg_exec : front == FRONT_DEPTH ? h->depth_exec : h->batch_exec)[a][m];
+  const int front_launches = front == FRONT_ORGANIZE ? 3 : front == FRONT_DEPTH ? 1 : 0;
   if (!exec)
   {
     const long long l0 = h->launches, f0 = h->prof_frames;
     cudaGraph_t g = nullptr;
     CK (cudaStreamBeginCapture (s, cudaStreamCaptureModeThreadLocal));
     int rc = B200TSDF_OK;
-    if (organize) rc = launch_organize (h, s, org_block (d_recs, m), org_recs (d_recs, m), m, org_keys (h), org_filled (h), org_images (h));
-    // (the first k_front of an unorganised batch reads what the gather wrote: no programmatic overlap with it, see launch_frame)
-    for (int i = 0; i < m && rc == B200TSDF_OK; ++i) rc = launch_frame (h, s, d_recs + i, false, !(organize && i == 0));
+    if (front == FRONT_ORGANIZE) rc = launch_organize (h, s, org_block (d_recs, m), org_recs (d_recs, m), m, org_keys (h), org_filled (h), org_images (h));
+    if (front == FRONT_DEPTH) rc = launch_depth (h, s, depth_block (d_recs, m), m, org_images (h));
+    // (the first k_front of an unorganised or depth batch reads what the front end wrote: no programmatic overlap with it, see
+    // launch_frame)
+    for (int i = 0; i < m && rc == B200TSDF_OK; ++i) rc = launch_frame (h, s, d_recs + i, false, !(front != FRONT_NONE && i == 0));
     cudaError_t ce = cudaStreamEndCapture (s, &g);
-    h->launches_per_frame = (int) ((h->launches - l0 - org_launches) / std::max (1, m));
+    h->launches_per_frame = (int) ((h->launches - l0 - front_launches) / std::max (1, m));
     h->launches = l0; h->prof_frames = f0;
     if (rc) { if (g) cudaGraphDestroy (g); return rc; }
     if (ce != cudaSuccess) return h->fail (B200TSDF_ECUDA, std::string ("graph capture: ") + cudaGetErrorString (ce));
@@ -1817,7 +1854,7 @@ static int batch_launch (b200tsdf* h, int m, bool organize = false)
   h->half_used[a] = true;
   note_device_err (h, s);
   h->bring_half ^= 1;
-  h->launches += org_launches + (long long) m * h->launches_per_frame; h->graph_launches++;
+  h->launches += front_launches + (long long) m * h->launches_per_frame; h->graph_launches++;
   h->prof_frames += m;
   h->timed = false;
   h->is_empty = false;
@@ -2027,7 +2064,7 @@ int unorganized_batches (b200tsdf* h, int n, const void* const* d_points, const 
     }
     FrameNumbering num (h);
     if (int rc = batch_records (h, m, imgs, 16, 0, 12, h->cfg.image_width, h->cfg.image_height, poses_c2w + 16 * (size_t) done, h->stream, &ob, recs)) return rc;
-    if (int rc = batch_launch (h, m, true)) return rc;
+    if (int rc = batch_launch (h, m, FRONT_ORGANIZE)) return rc;
     num.enqueued = true;
     done += m;
   }
@@ -2098,6 +2135,154 @@ int b200tsdf_integrate_unorganized_batch_device (b200tsdf_t* h, int n, const voi
   cudaSetDevice (h->device);
   if (int rc = pending_device_err (h)) return rc;
   return unorganized_batches (h, n, d_points, counts, stride, xyz_off, rgba_off, opts, poses_c2w);
+}
+
+// ---- depth images (depth.cuh, DESIGN.md §3h) ----------------------------------------------------
+// A depth frame is one integrateCloud of the organised cloud depth_pixel makes from it: the batch's depth block travels behind
+// its frame records, k_depth_unproject writes the images of the unorganised batch path (org_images), and the frames fuse from
+// there, m frames per record half, each half one graph launch.
+namespace {
+
+// the checks every depth entry point applies before anything is enqueued
+int depth_args (b200tsdf* h, int format, float scale, int width, int height)
+{
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "depth image before reset() (the image size and intrinsics are read at reset)");
+  if (h->p.shard_count > 1 || h->comm) return h->fail (B200TSDF_ESTATE, "depth images on a shard: integrate them on an unsharded handle");
+  if (format != B200TSDF_DEPTH_U16 && format != B200TSDF_DEPTH_F32) return h->fail (B200TSDF_EINVAL, "bad depth format");
+  if (!(scale > 0.f && scale <= 3.402823466e38f)) return h->fail (B200TSDF_EINVAL, "depth scale must be finite and > 0");
+  if (width != h->cfg.image_width || height != h->cfg.image_height)
+    return h->fail (B200TSDF_EINVAL, "depth image size differs from setImageSize() (the intrinsics belong to that size)");
+  return B200TSDF_OK;
+}
+
+size_t depth_elem (int format) { return format == B200TSDF_DEPTH_U16 ? 2 : 4; }
+
+int depth_ptr (b200tsdf* h, const void* depth, int format)
+{
+  if (!depth) return h->fail (B200TSDF_EINVAL, "null depth image");
+  if (reinterpret_cast<uintptr_t> (depth) % depth_elem (format)) return h->fail (B200TSDF_EINVAL, "depth image not aligned to its element size");
+  return B200TSDF_OK;
+}
+
+DepthBatch depth_batch (const b200tsdf* h, int format, float scale)
+{
+  DepthBatch b{};
+  b.fx = (float) h->cfg.fx; b.fy = (float) h->cfg.fy; b.cx = (float) h->cfg.cx; b.cy = (float) h->cfg.cy;
+  b.scale = scale; b.width = h->cfg.image_width; b.height = h->cfg.image_height; b.format = format;
+  return b;
+}
+
+// n depth frames resident in device memory, HALF per record half.  The arguments have been checked and org_buffers sized.
+// A colour image on a volume without colour is not read (the frame fuses with rgba_off = -1, as a cloud's colour would be
+// ignored there).
+int depth_batches (b200tsdf* h, int n, const void* const* d_depth, int format, float scale, const void* const* d_rgb, const double* poses_c2w)
+{
+  constexpr int HALF = FRAME_RING / 2;
+  const bool color = h->p.color && d_rgb;
+  DepthBatch db = depth_batch (h, format, scale);
+  const size_t npix = org_npix (h);
+  for (int done = 0; done < n;)
+  {
+    const int m = std::min (HALF, n - done);
+    const void* imgs[HALF];
+    for (int i = 0; i < m; ++i)
+    {
+      imgs[i] = org_images (h) + (size_t) i * npix * 16;
+      db.depth[i] = d_depth[done + i];
+      db.rgb[i] = color ? static_cast<const unsigned char*> (d_rgb[done + i]) : nullptr;
+    }
+    FrameNumbering num (h);
+    if (int rc = batch_records (h, m, imgs, 16, 0, color ? 12 : -1, h->cfg.image_width, h->cfg.image_height, poses_c2w + 16 * (size_t) done,
+                                h->stream, nullptr, nullptr, &db)) return rc;
+    if (int rc = batch_launch (h, m, FRONT_DEPTH)) return rc;
+    num.enqueued = true;
+    done += m;
+  }
+  CK (cudaGetLastError ());
+  return B200TSDF_OK;
+}
+
+} // namespace
+
+int b200tsdf_integrate_depth (b200tsdf_t* h, const void* depth, int depth_format, float depth_scale, const uint8_t* rgb,
+                              int width, int height, const double* pose_c2w)
+{
+  if (!h || !pose_c2w) return B200TSDF_EINVAL;
+  if (int rc = depth_args (h, depth_format, depth_scale, width, height)) return rc;
+  if (int rc = depth_ptr (h, depth, depth_format)) return rc;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  if (int rc = org_buffers (h)) return rc;
+  const size_t npix = org_npix (h), dbytes = npix * depth_elem (depth_format), cbytes = rgb && h->p.color ? npix * 3 : 0;
+  const size_t slot_bytes = npix * 7;                                 // the widest frame: float32 depth and colour
+  if (!h->h_depth[0].p || h->h_depth[0].bytes < slot_bytes || h->d_depth_raw[0].cap < slot_bytes)
+  {
+    CK (cudaStreamSynchronize (h->stream)); CK (cudaStreamSynchronize (h->copy_stream));
+    for (int i = 0; i < DEPTH_SLOTS; ++i)
+    {
+      if (h->h_depth[i].alloc (slot_bytes)) { for (int k = 0; k < DEPTH_SLOTS; ++k) h->h_depth[k].release (); return alloc_failed (h, "pinned staging of depth images"); }
+      if (h->d_depth_raw[i].grow (slot_bytes)) return alloc_failed (h, "device buffers of depth images");
+    }
+    h->depth_no = 0;
+  }
+  // the slot's last upload has run (so its staging is free), and that upload's unprojection has read the device buffer
+  // before the next upload rewrites it; fusion of earlier frames is never waited for here
+  const int b = (int) (h->depth_no % DEPTH_SLOTS);
+  if (h->depth_no >= (uint64_t) DEPTH_SLOTS)
+  {
+    CK (cudaEventSynchronize (h->ev_dcopied[b]));
+    CK (cudaStreamWaitEvent (h->copy_stream, h->ev_dconsumed[b], 0));
+  }
+  unsigned char* stage = h->h_depth[b].p;
+  std::memcpy (stage, depth, dbytes);                                 // the caller's buffers are free when this call returns
+  if (cbytes) std::memcpy (stage + dbytes, rgb, cbytes);
+  unsigned char* d_raw = h->d_depth_raw[b];
+  CK (cudaMemcpyAsync (d_raw, stage, dbytes + cbytes, cudaMemcpyHostToDevice, h->copy_stream));
+  h->h2d_bytes += (long long) (dbytes + cbytes);
+  CK (cudaEventRecord (h->ev_dcopied[b], h->copy_stream));
+  CK (cudaStreamWaitEvent (h->stream, h->ev_dcopied[b], 0));
+  const void* d_depth = d_raw;
+  const void* d_rgb = d_raw + dbytes;
+  if (int rc = depth_batches (h, 1, &d_depth, depth_format, depth_scale, cbytes ? &d_rgb : nullptr, pose_c2w)) return rc;
+  CK (cudaEventRecord (h->ev_dconsumed[b], h->stream));
+  h->depth_no++;
+  return B200TSDF_OK;
+}
+
+int b200tsdf_integrate_depth_batch_device (b200tsdf_t* h, int n, const void* const* d_depth, int depth_format, float depth_scale,
+                                           const void* const* d_rgb, int width, int height, const double* poses_c2w)
+{
+  if (!h || n < 0 || (n && (!d_depth || !poses_c2w))) return B200TSDF_EINVAL;
+  if (int rc = depth_args (h, depth_format, depth_scale, width, height)) return rc;
+  // every pointer of every record half, before any frame is numbered: a refused batch enqueues nothing
+  for (int i = 0; i < n; ++i)
+  {
+    if (int rc = depth_ptr (h, d_depth[i], depth_format)) return rc;
+    if (d_rgb && !d_rgb[i]) return h->fail (B200TSDF_EINVAL, "null colour image in batch");
+  }
+  if (!n) return B200TSDF_OK;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  if (int rc = org_buffers (h)) return rc;
+  return depth_batches (h, n, d_depth, depth_format, depth_scale, d_rgb, poses_c2w);
+}
+
+int b200tsdf_depth_to_cloud_device (b200tsdf_t* h, const void* d_depth, int depth_format, float depth_scale, const uint8_t* d_rgb,
+                                    int width, int height, void* d_out)
+{
+  if (!h) return B200TSDF_EINVAL;
+  if (int rc = depth_args (h, depth_format, depth_scale, width, height)) return rc;
+  if (int rc = depth_ptr (h, d_depth, depth_format)) return rc;
+  if (!d_out || reinterpret_cast<uintptr_t> (d_out) % 16) return h->fail (B200TSDF_EINVAL, "output image null or not 16-byte aligned");
+  cudaSetDevice (h->device);
+  if (int rc = h->scratch (sizeof (DepthBatch))) return rc;
+  DepthBatch db = depth_batch (h, depth_format, depth_scale);
+  db.depth[0] = d_depth; db.rgb[0] = d_rgb;
+  cudaStream_t s = h->stream;
+  CK (cudaMemcpyAsync (h->d_scratch, &db, sizeof (db), cudaMemcpyHostToDevice, s));          // (pageable: staged before the call returns)
+  if (int rc = launch_depth (h, s, reinterpret_cast<const DepthBatch*> (h->d_scratch.p), 1, static_cast<unsigned char*> (d_out))) return rc;
+  CK (cudaStreamSynchronize (s));
+  return B200TSDF_OK;
 }
 
 int b200tsdf_sync (b200tsdf_t* h)

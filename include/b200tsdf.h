@@ -174,6 +174,35 @@ int  b200tsdf_integrate_unorganized_batch_device (b200tsdf_t* h, int n, const vo
                                                   size_t stride, int xyz_off, int rgba_off,
                                                   const b200tsdf_organize_opts* opts, const double* poses_c2w);
 
+/* ---- depth images ----
+ * A depth frame is exactly one integrateCloud of the organised cloud it unprojects to.  For pixel (u, v) of a row-major
+ * width x height depth map D, with the handle's intrinsics rounded to float, each operation a float32 operation rounded to
+ * nearest:  z = (float) D[v*width + u] * depth_scale;  x = ((float) u - cx) * z / fx;  y = ((float) v - cy) * z / fy.
+ * A pixel with D == 0 or z not finite (NaN / inf input, overflow) is invalid: x = y = z = NaN.  Negative z passes through.
+ * rgb (optional): a registered image of 3 bytes per pixel, R, G, B, same size; it becomes the PCL colour bytes b, g, r, 255
+ * (0, 0, 0, 255 without one) and is ignored by a volume without colour.  width x height must be the configured image size;
+ * images are contiguous.  Refused with B200TSDF_EINVAL, nothing enqueued and the handle unchanged: a bad format, a scale that
+ * is not finite or <= 0, another size, a NULL depth pointer (in a batch: any of them, or a NULL entry of d_rgb), a depth
+ * pointer not aligned to its element size.  B200TSDF_ESTATE before reset() and on a sharded handle; B200TSDF_ENOMEM when the
+ * images of one batch (32 * image_width * image_height * 24 bytes, shared with the unorganised batches) do not fit. */
+#define B200TSDF_DEPTH_U16  1   /* uint16_t in sensor units (depth_scale metres per unit, e.g. 1e-3) */
+#define B200TSDF_DEPTH_F32  2   /* float                                                          */
+/* one depth frame from host memory.  The caller's buffers are free when the call returns; the call waits only for the
+ * handle's own staging (a small ring of pinned slots), never for the fusion of earlier frames, so the upload of frame i+1
+ * overlaps the fusion of frame i.  Errors of the fusion are reported as for b200tsdf_integrate_device. */
+int  b200tsdf_integrate_depth (b200tsdf_t* h, const void* depth, int depth_format, float depth_scale, const uint8_t* rgb,
+                               int width, int height, const double* pose_c2w);
+/* n consecutive b200tsdf_integrate_depth calls on images resident in device memory of h's device (d_depth: n device
+ * pointers; d_rgb: NULL or n device pointers; poses_c2w: n row-major 4x4 matrices back to back).  Every 32 frames are
+ * unprojected and fused by one CUDA-graph launch.  Asynchronous like b200tsdf_integrate_batch_device. */
+int  b200tsdf_integrate_depth_batch_device (b200tsdf_t* h, int n, const void* const* d_depth, int depth_format, float depth_scale,
+                                            const void* const* d_rgb, int width, int height, const double* poses_c2w);
+/* the organised cloud of one depth frame (device memory) written to d_out as 16-byte pixels {x, y, z, bgra} (device memory,
+ * 16-byte aligned, width * height * 16 bytes); the colour word is written whether or not the volume has colour.  Returns when
+ * the image is written. */
+int  b200tsdf_depth_to_cloud_device (b200tsdf_t* h, const void* d_depth, int depth_format, float depth_scale, const uint8_t* d_rgb,
+                                     int width, int height, void* d_out);
+
 /* getFxn / getGradient / getHessian (cpp:655-725) with mode 0, or the combined
  * getFxnAndGradient / getFxnGradientAndHessian (cpp:728-794) with mode 1.  what: bit0 value,
  * bit1 gradient (3 floats), bit2 hessian (9 floats, row-major).  ok[i] = the reference's bool; where it is 0 the outputs of

@@ -226,6 +226,30 @@ public:
     return status_ == 0;
   }
 
+  // extension: one depth frame from host memory, exactly integrateCloud of the organised cloud it unprojects to
+  // (b200tsdf_integrate_depth): a width x height map, the configured image size, of uint16 sensor units times `scale` metres
+  // or of float metres, and an optional registered image of 3 bytes per pixel, R, G, B.  The buffers are free on return.
+  bool integrateDepthImage (const std::uint16_t* depth, float scale, int width, int height, const Affine3d& trans = Affine3d::Identity (),
+                            const std::uint8_t* rgb = nullptr)
+  { return depth_image (depth, B200TSDF_DEPTH_U16, scale, width, height, trans, rgb); }
+  bool integrateDepthImage (const float* depth, int width, int height, const Affine3d& trans = Affine3d::Identity (),
+                            const std::uint8_t* rgb = nullptr)
+  { return depth_image (depth, B200TSDF_DEPTH_F32, 1.f, width, height, trans, rgb); }
+  // integrateDepthImage for every map of a batch resident in device memory (format B200TSDF_DEPTH_U16 or _F32; d_rgb empty or
+  // one image per map), with the same result.  Asynchronous on the volume's stream: every 32 maps are one CUDA-graph launch.
+  bool integrateDepthImagesDevice (const std::vector<const void*>& d_depth, int format, float scale, int width, int height,
+                                   const std::vector<Affine3d>& poses, const std::vector<const void*>& d_rgb = {})
+  {
+    if (!h_) return false;
+    const std::size_t n = d_depth.size ();
+    if (poses.size () != n || (!d_rgb.empty () && d_rgb.size () != n)) { status_ = B200TSDF_EINVAL; return false; }
+    std::vector<double> m (16 * n);
+    for (std::size_t i = 0; i < n; ++i) detail::pose_rows (poses[i], m.data () + 16 * i);
+    status_ = b200tsdf_integrate_depth_batch_device (h_, static_cast<int> (n), d_depth.data (), format, scale,
+                                                     d_rgb.empty () ? nullptr : d_rgb.data (), width, height, m.data ());
+    return status_ == 0;
+  }
+
   bool getFxn (const PointXYZ& pt, float& val) const                                               // cpp:655-672
   { std::uint8_t ok = 0; float p[3] = { pt.x, pt.y, pt.z }; b200tsdf_query (h_, p, 1, 1, 0, &val, nullptr, nullptr, &ok); return ok != 0; }
   bool getGradient (const PointXYZ& pt, float grad[3]) const                                       // cpp:681-700
@@ -451,6 +475,14 @@ public:
 
 private:
   void push () { if (h_) status_ = b200tsdf_set_config (h_, &cfg_); }
+  bool depth_image (const void* depth, int format, float scale, int width, int height, const Affine3d& trans, const std::uint8_t* rgb)
+  {
+    if (!h_) return false;
+    double m[16];
+    detail::pose_rows (trans, m);
+    status_ = b200tsdf_integrate_depth (h_, depth, format, scale, rgb, width, height, m);
+    return status_ == 0;
+  }
   int num_random_splits_ = 1;
   b200tsdf_config cfg_{};
   b200tsdf_t* h_ = nullptr;
