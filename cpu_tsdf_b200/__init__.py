@@ -84,6 +84,7 @@ EXPORTS = [
     "b200tsdf_set_containing_voxels", "b200tsdf_set_containing_voxels_device",
     "b200tsdf_changed_cells", "b200tsdf_mesh_cells_device",
     "b200tsdf_integrate_depth", "b200tsdf_integrate_depth_batch_device", "b200tsdf_depth_to_cloud_device",
+    "b200tsdf_default_track_params", "b200tsdf_track_depth", "b200tsdf_track_depth_device", "b200tsdf_track_cloud_device",
 ]
 
 # depth formats of the depth-image entry points (B200TSDF_DEPTH_*)
@@ -94,6 +95,44 @@ DEPTH_F32 = 2
 VOXEL_DTYPE = np.dtype([("level", "<i4"), ("x", "<i4"), ("y", "<i4"), ("z", "<i4"),
                         ("cx", "<f4"), ("cy", "<f4"), ("cz", "<f4"), ("size", "<f4"),
                         ("d", "<f4"), ("w", "<f4"), ("r", "u1"), ("g", "u1"), ("b", "u1"), ("has_children", "u1")])
+
+
+# status of a tracking call (B200TSDF_TRACK_*)
+TRACK_CONVERGED = 0
+TRACK_MAX_ITERS = 1
+TRACK_TOO_FEW_INLIERS = 2
+TRACK_SINGULAR = 3
+
+
+class TrackParams(C.Structure):
+    """b200tsdf_track_params (include/b200tsdf.h); TrackParams.default() holds b200tsdf_default_track_params"""
+    _fields_ = [("levels", C.c_int32), ("stride", C.c_int32 * 4), ("iters", C.c_int32 * 4),
+                ("huber_delta", C.c_float), ("d_max", C.c_float), ("w_min", C.c_float), ("min_inliers", C.c_int32),
+                ("damping", C.c_double), ("eps_rot", C.c_double), ("eps_trans", C.c_double)]
+
+    @classmethod
+    def default(cls, **kw):
+        p = cls()
+        load_library().b200tsdf_default_track_params(C.byref(p))
+        for k, v in kw.items():
+            if k in ("stride", "iters"):
+                v = list(v) + [0] * (4 - len(v))
+                getattr(p, k)[:] = [int(x) for x in v]
+            elif not hasattr(p, k):
+                raise AttributeError(k)
+            else:
+                setattr(p, k, v)
+        return p
+
+
+class TrackResult(C.Structure):
+    """b200tsdf_track_result (include/b200tsdf.h)"""
+    _fields_ = [("pose_c2w", C.c_double * 16), ("status", C.c_int32), ("iters", C.c_int32 * 4), ("inliers", C.c_int32),
+                ("n_log", C.c_int32), ("reserved", C.c_int32), ("rms", C.c_double), ("A", C.c_double * 36), ("b", C.c_double * 6)]
+
+
+# b200tsdf_track_iter: one iteration of a tracking call's log
+TRACK_ITER_DTYPE = np.dtype([("level", "<i4"), ("inliers", "<i4"), ("cost", "<f8"), ("step", "<f8", (6,))])
 
 
 class Voxel(C.Structure):
@@ -147,6 +186,11 @@ def load_library() -> C.CDLL:
     lib.b200tsdf_integrate_depth.argtypes = [vp, vp, C.c_int, C.c_float, vp, C.c_int, C.c_int, vp]
     lib.b200tsdf_integrate_depth_batch_device.argtypes = [vp, C.c_int, vp, C.c_int, C.c_float, vp, C.c_int, C.c_int, vp]
     lib.b200tsdf_depth_to_cloud_device.argtypes = [vp, vp, C.c_int, C.c_float, vp, C.c_int, C.c_int, vp]
+    tp, tr = C.POINTER(TrackParams), C.POINTER(TrackResult)
+    lib.b200tsdf_default_track_params.argtypes = [tp]; lib.b200tsdf_default_track_params.restype = None
+    lib.b200tsdf_track_depth.argtypes = [vp, vp, C.c_int, C.c_float, C.c_int, C.c_int, vp, tp, tr, vp]
+    lib.b200tsdf_track_depth_device.argtypes = [vp, vp, C.c_int, C.c_float, C.c_int, C.c_int, vp, tp, tr, vp]
+    lib.b200tsdf_track_cloud_device.argtypes = [vp, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, vp, tp, tr, vp]
     lib.b200tsdf_query.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.b200tsdf_interpolate.argtypes = [vp, vp, C.c_int, vp, vp]
     lib.b200tsdf_render.argtypes = [vp, vp, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, vp]
@@ -520,6 +564,56 @@ class TSDFVolumeOctree:
         dp = lambda x: C.c_void_p(int(x)) if x else None
         self._check(self._lib.b200tsdf_depth_to_cloud_device(self._h, dp(d_depth), int(depth_format), float(depth_scale), dp(d_rgb),
                                                              W, H, dp(d_out)))
+
+    # ---- tracking (DESIGN.md §3i) ----
+    def _track(self, call, params):
+        prm = TrackParams.default() if params is None else params
+        res = TrackResult()
+        log = np.zeros(max(1, sum(prm.iters[:max(1, min(4, prm.levels))])), TRACK_ITER_DTYPE)
+        self._check(call(C.byref(prm), C.byref(res), log.ctypes.data_as(C.c_void_p)))
+        result = {
+            "status": int(res.status), "iters": list(res.iters), "inliers": int(res.inliers), "rms": float(res.rms),
+            "A": np.array(res.A, np.float64).reshape(6, 6), "b": np.array(res.b, np.float64),
+            "log": log[:res.n_log].copy(),
+        }
+        return np.array(res.pose_c2w, np.float64).reshape(4, 4), result
+
+    def trackDepth(self, depth: np.ndarray, pose0, params: "TrackParams | None" = None, depth_scale=1e-3):
+        """Refine the camera->world pose of one depth frame ([H, W] uint16 or float32 in host memory, the configured image size)
+        against the volume, from pose0, by point-to-SDF Gauss-Newton (b200tsdf_track_depth).  The volume is only read.
+        Returns (pose [4, 4] float64, result dict: status (TRACK_*), iters per level, inliers, rms, A [6, 6], b [6], log)."""
+        d = np.ascontiguousarray(depth)
+        if d.dtype == np.uint16:
+            fmt = DEPTH_U16
+        elif d.dtype == np.float32:
+            fmt = DEPTH_F32
+        else:
+            raise ValueError("depth must be uint16 or float32")
+        if d.ndim != 2:
+            raise ValueError("depth must be [H, W]")
+        pose = _pose(pose0)
+        return self._track(lambda p, r, lg: self._lib.b200tsdf_track_depth(self._h, _ptr(d), fmt, float(depth_scale), d.shape[1], d.shape[0],
+                                                                          _ptr(pose), p, r, lg), params)
+
+    def trackDepthDevice(self, d_depth, pose0, params: "TrackParams | None" = None, *, depth_format: int, depth_scale: float,
+                         width: int | None = None, height: int | None = None):
+        """trackDepth on a depth map resident in device memory (an integer device pointer)"""
+        W = self._cfg.image_width if width is None else width
+        H = self._cfg.image_height if height is None else height
+        pose = _pose(pose0)
+        dp = C.c_void_p(int(d_depth)) if d_depth else None
+        return self._track(lambda p, r, lg: self._lib.b200tsdf_track_depth_device(self._h, dp, int(depth_format), float(depth_scale), W, H,
+                                                                                 _ptr(pose), p, r, lg), params)
+
+    def trackCloudDevice(self, d_points, pose0, params: "TrackParams | None" = None, *, stride: int = 16, xyz_off: int = 0,
+                         width: int | None = None, height: int | None = None):
+        """trackDepth on an organised cloud resident in device memory, in integrateCloudDevice's layout (colour is not read)"""
+        W = self._cfg.image_width if width is None else width
+        H = self._cfg.image_height if height is None else height
+        pose = _pose(pose0)
+        dp = C.c_void_p(int(d_points)) if d_points else None
+        return self._track(lambda p, r, lg: self._lib.b200tsdf_track_cloud_device(self._h, dp, int(stride), int(xyz_off), W, H,
+                                                                                 _ptr(pose), p, r, lg), params)
 
     def _query(self, pts, what, mode):
         xyz = np.ascontiguousarray(pts, dtype=np.float32).reshape(-1, 3)

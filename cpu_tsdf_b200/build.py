@@ -10,7 +10,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200tsdf.so")
 # source -> headers it includes (csrc/), for incremental rebuilds
 SOURCES = {
-    "engine.cu": ["tsdf_core.cuh", "mc_tables.cuh", "host_math.h", "params_setup.h", "brick_kernels.cuh", "obs_fast.cuh", "brick_direct.cuh", "multigpu.cuh", "organize.cuh", "mesh_sort.h", "host_pack.h", "vol_io.cuh", "pool_rehash.cuh", "depth.cuh"],
+    "engine.cu": ["tsdf_core.cuh", "mc_tables.cuh", "host_math.h", "params_setup.h", "brick_kernels.cuh", "obs_fast.cuh", "brick_direct.cuh", "multigpu.cuh", "organize.cuh", "mesh_sort.h", "host_pack.h", "vol_io.cuh", "pool_rehash.cuh", "depth.cuh", "track.cuh"],
     "meshpost.cu": ["tsdf_core.cuh", "meshpost_core.cuh", "mesh_sort.h"],
 }
 OBJ = os.path.join(CSRC, "_obj")

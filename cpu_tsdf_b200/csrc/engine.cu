@@ -11,6 +11,7 @@
 #include "brick_direct.cuh"
 #include "organize.cuh"
 #include "depth.cuh"
+#include "track.cuh"
 #include "mesh_sort.h"
 #include "host_pack.h"
 #include "vol_io.cuh"
@@ -21,6 +22,8 @@
 #include <sys/syscall.h>
 #include <unistd.h>
 #include <algorithm>
+#include <cmath>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -1059,6 +1062,11 @@ struct b200tsdf
   Staging h_depth[DEPTH_SLOTS]; DevBuf<unsigned char> d_depth_raw[DEPTH_SLOTS];
   Event ev_dcopied[DEPTH_SLOTS], ev_dconsumed[DEPTH_SLOTS];
   uint64_t depth_no = 0;
+  // tracking (track.cuh): one block of inputs and state per call (pinned image and device copy), the per-tile sums of the
+  // finest possible level, and one captured graph per (schedule shape, input kind), dropped with the batch graphs
+  Pinned<TrackBlock> h_track; DevBuf<TrackBlock> d_track; DevBuf<double> d_track_part;
+  struct TrackGraph { int key[10]; cudaGraphExec_t exec; };
+  std::vector<TrackGraph> track_exec;
   // multi-GPU (multigpu.cuh): NCCL communicator (opaque here), row-sliced uploads
   void* comm = nullptr; int comm_rank = 0, comm_size = 1;
   DevBuf<unsigned char> d_rows_raw[2], d_rows_full[2];
@@ -1138,6 +1146,12 @@ cudaError_t launch_pdl (void (*kernel) (KArgs...), dim3 grid, dim3 block, cudaSt
 
 void comm_release (b200tsdf* h);          // multigpu.cuh
 
+void drop_track_graphs (b200tsdf* h)
+{
+  for (auto& g : h->track_exec) cudaGraphExecDestroy (g.exec);
+  h->track_exec.clear ();
+}
+
 void drop_batch_graphs (b200tsdf* h)
 {
   for (int a = 0; a < 2; ++a)
@@ -1147,6 +1161,7 @@ void drop_batch_graphs (b200tsdf* h)
       if (h->unorg_exec[a][n]) { cudaGraphExecDestroy (h->unorg_exec[a][n]); h->unorg_exec[a][n] = nullptr; }
       if (h->depth_exec[a][n]) { cudaGraphExecDestroy (h->depth_exec[a][n]); h->depth_exec[a][n] = nullptr; }
     }
+  drop_track_graphs (h);
 }
 
 int check_device_err (b200tsdf* h)
@@ -2202,19 +2217,12 @@ int depth_batches (b200tsdf* h, int n, const void* const* d_depth, int format, f
   return B200TSDF_OK;
 }
 
-} // namespace
-
-int b200tsdf_integrate_depth (b200tsdf_t* h, const void* depth, int depth_format, float depth_scale, const uint8_t* rgb,
-                              int width, int height, const double* pose_c2w)
+// The caller's depth (dbytes) and colour (cbytes, 0: none) copied into pinned slot b and uploaded on copy_stream into that
+// slot's device buffer d_raw; the handle's stream waits for the upload.  The caller records ev_dconsumed[b] on the stream
+// behind the last launch that reads d_raw, and advances depth_no.
+int stage_depth (b200tsdf* h, const void* depth, size_t dbytes, const uint8_t* rgb, size_t cbytes, int& b, unsigned char*& d_raw)
 {
-  if (!h || !pose_c2w) return B200TSDF_EINVAL;
-  if (int rc = depth_args (h, depth_format, depth_scale, width, height)) return rc;
-  if (int rc = depth_ptr (h, depth, depth_format)) return rc;
-  cudaSetDevice (h->device);
-  if (int rc = pending_device_err (h)) return rc;
-  if (int rc = org_buffers (h)) return rc;
-  const size_t npix = org_npix (h), dbytes = npix * depth_elem (depth_format), cbytes = rgb && h->p.color ? npix * 3 : 0;
-  const size_t slot_bytes = npix * 7;                                 // the widest frame: float32 depth and colour
+  const size_t slot_bytes = org_npix (h) * 7;                         // the widest frame: float32 depth and colour
   if (!h->h_depth[0].p || h->h_depth[0].bytes < slot_bytes || h->d_depth_raw[0].cap < slot_bytes)
   {
     CK (cudaStreamSynchronize (h->stream)); CK (cudaStreamSynchronize (h->copy_stream));
@@ -2227,7 +2235,7 @@ int b200tsdf_integrate_depth (b200tsdf_t* h, const void* depth, int depth_format
   }
   // the slot's last upload has run (so its staging is free), and that upload's unprojection has read the device buffer
   // before the next upload rewrites it; fusion of earlier frames is never waited for here
-  const int b = (int) (h->depth_no % DEPTH_SLOTS);
+  b = (int) (h->depth_no % DEPTH_SLOTS);
   if (h->depth_no >= (uint64_t) DEPTH_SLOTS)
   {
     CK (cudaEventSynchronize (h->ev_dcopied[b]));
@@ -2236,11 +2244,29 @@ int b200tsdf_integrate_depth (b200tsdf_t* h, const void* depth, int depth_format
   unsigned char* stage = h->h_depth[b].p;
   std::memcpy (stage, depth, dbytes);                                 // the caller's buffers are free when this call returns
   if (cbytes) std::memcpy (stage + dbytes, rgb, cbytes);
-  unsigned char* d_raw = h->d_depth_raw[b];
+  d_raw = h->d_depth_raw[b];
   CK (cudaMemcpyAsync (d_raw, stage, dbytes + cbytes, cudaMemcpyHostToDevice, h->copy_stream));
   h->h2d_bytes += (long long) (dbytes + cbytes);
   CK (cudaEventRecord (h->ev_dcopied[b], h->copy_stream));
   CK (cudaStreamWaitEvent (h->stream, h->ev_dcopied[b], 0));
+  return B200TSDF_OK;
+}
+
+} // namespace
+
+int b200tsdf_integrate_depth (b200tsdf_t* h, const void* depth, int depth_format, float depth_scale, const uint8_t* rgb,
+                              int width, int height, const double* pose_c2w)
+{
+  if (!h || !pose_c2w) return B200TSDF_EINVAL;
+  if (int rc = depth_args (h, depth_format, depth_scale, width, height)) return rc;
+  if (int rc = depth_ptr (h, depth, depth_format)) return rc;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  if (int rc = org_buffers (h)) return rc;
+  const size_t npix = org_npix (h), dbytes = npix * depth_elem (depth_format), cbytes = rgb && h->p.color ? npix * 3 : 0;
+  int b = 0;
+  unsigned char* d_raw = nullptr;
+  if (int rc = stage_depth (h, depth, dbytes, rgb, cbytes, b, d_raw)) return rc;
   const void* d_depth = d_raw;
   const void* d_rgb = d_raw + dbytes;
   if (int rc = depth_batches (h, 1, &d_depth, depth_format, depth_scale, cbytes ? &d_rgb : nullptr, pose_c2w)) return rc;
@@ -2283,6 +2309,199 @@ int b200tsdf_depth_to_cloud_device (b200tsdf_t* h, const void* d_depth, int dept
   if (int rc = launch_depth (h, s, reinterpret_cast<const DepthBatch*> (h->d_scratch.p), 1, static_cast<unsigned char*> (d_out))) return rc;
   CK (cudaStreamSynchronize (s));
   return B200TSDF_OK;
+}
+
+// ---- tracking (track.cuh, DESIGN.md §3i) -------------------------------------------------------------------------------
+// One call: the inputs and the initial state go up in one copy, the captured graph of the schedule runs (the depth
+// unprojection first for a depth map, then k_track_terms and k_track_solve per iteration; once a level has converged or the
+// call has stopped, the remaining launches return at once), and the state comes back in one copy behind it.
+namespace {
+
+constexpr int TRACK_GRAPHS = 8;   // captured schedules kept per handle (the oldest goes first)
+
+int track_args (b200tsdf* h, const double* pose0, const b200tsdf_track_params* prm, const b200tsdf_track_result* res)
+{
+  if (!h->has_volume) return h->fail (B200TSDF_ESTATE, "tracking before reset()");
+  if (h->p.shard_count > 1 || h->comm) return h->fail (B200TSDF_ESTATE, "tracking on a shard: track against an unsharded handle");
+  if (!pose0 || !prm || !res) return h->fail (B200TSDF_EINVAL, "null pose, tracking parameters or result");
+  for (int i = 0; i < 16; ++i)
+    if (!std::isfinite (pose0[i])) return h->fail (B200TSDF_EINVAL, "initial pose not finite");
+  if (prm->levels < 1 || prm->levels > TRACK_LEVELS) return h->fail (B200TSDF_EINVAL, "tracking levels outside 1..4");
+  for (int l = 0; l < prm->levels; ++l)
+  {
+    if (prm->stride[l] < 1) return h->fail (B200TSDF_EINVAL, "tracking stride < 1");
+    if (prm->iters[l] < 0 || prm->iters[l] > TRACK_MAX_ITERS) return h->fail (B200TSDF_EINVAL, "tracking iterations outside 0..64");
+  }
+  if (!(prm->huber_delta > 0.f && std::isfinite (prm->huber_delta)) || !(prm->d_max > 0.f) || !std::isfinite (prm->w_min))
+    return h->fail (B200TSDF_EINVAL, "huber_delta and d_max must be > 0 (huber_delta finite), w_min finite");
+  if (!(prm->damping >= 0.0 && std::isfinite (prm->damping)) || !(prm->eps_rot >= 0.0 && std::isfinite (prm->eps_rot))
+      || !(prm->eps_trans >= 0.0 && std::isfinite (prm->eps_trans)) || prm->min_inliers < 0)
+    return h->fail (B200TSDF_EINVAL, "damping, eps_rot and eps_trans must be finite and >= 0, min_inliers >= 0");
+  return B200TSDF_OK;
+}
+
+TrackInput track_input (const b200tsdf* h, const b200tsdf_track_params* prm, const void* pts, size_t stride, int xyz_off)
+{
+  TrackInput in{};
+  in.pts = static_cast<const unsigned char*> (pts); in.stride = (int) stride; in.xyz_off = xyz_off;
+  in.width = h->cfg.image_width; in.height = h->cfg.image_height;
+  in.levels = prm->levels; in.min_inliers = prm->min_inliers;
+  in.huber = prm->huber_delta; in.d_max = prm->d_max; in.w_min = prm->w_min;
+  in.damping = prm->damping; in.eps_rot = prm->eps_rot; in.eps_trans = prm->eps_trans;
+  return in;
+}
+
+// the launches of one schedule on stream s (being captured)
+void track_enqueue (b200tsdf* h, cudaStream_t s, bool depth, const b200tsdf_track_params* prm, int cap)
+{
+  TrackBlock* blk = h->d_track;
+  const int W = h->cfg.image_width, H = h->cfg.image_height;
+  if (depth) k_depth_unproject<<<dim3 ((unsigned) ((org_npix (h) + 255) / 256), 1), 256, 0, s>>> (&blk->db, (int) org_npix (h), org_images (h));
+  for (int l = 0; l < prm->levels; ++l)
+  {
+    const int tiles = (track_samples (W, H, prm->stride[l]) + TRACK_TILE - 1) / TRACK_TILE;
+    for (int k = 0; k < prm->iters[l]; ++k)
+    {
+      k_track_terms<<<tiles, TRACK_BLOCK, 0, s>>> (h->p, blk, l, prm->stride[l], h->d_track_part, cap);
+      k_track_solve<<<1, 32, 0, s>>> (blk, l, tiles, h->d_track_part, cap);
+    }
+  }
+}
+
+// The arguments have been checked; in.pts is the cloud (for a depth map, the organised image db unprojects into).  dslot >= 0:
+// a host depth map staged in that slot, released behind the unprojection.
+int track_run (b200tsdf* h, const TrackInput& in, const DepthBatch* db, int dslot, const double* pose0, const b200tsdf_track_params* prm,
+               b200tsdf_track_result* res, b200tsdf_track_iter* log)
+{
+  cudaStream_t s = h->stream;
+  const int cap = (track_samples (h->cfg.image_width, h->cfg.image_height, 1) + TRACK_TILE - 1) / TRACK_TILE;
+  if (!h->h_track.p && h->h_track.alloc (1)) { h->h_track.p = nullptr; return alloc_failed (h, "pinned tracking block"); }
+  if (h->d_track.grow (1)) return alloc_failed (h, "tracking block");
+  if (h->d_track_part.cap < (size_t) cap * TRACK_NS)
+  {
+    drop_track_graphs (h);                                   // (the captured schedules name the old buffer)
+    if (h->d_track_part.grow ((size_t) cap * TRACK_NS)) return alloc_failed (h, "tracking tile sums");
+  }
+  TrackBlock& B = *h->h_track.p;
+  B.in = in;
+  if (db) B.db = *db;
+  std::memset (&B.st, 0, sizeof (TrackState));
+  track_set_pose (B.st, pose0);
+  CK (cudaMemcpyAsync (h->d_track.p, &B, offsetof (TrackBlock, st) + offsetof (TrackState, log), cudaMemcpyHostToDevice, s));
+  int total = 0;
+  for (int l = 0; l < prm->levels; ++l) total += prm->iters[l];
+  if (total)
+  {
+    int key[10] = { db ? 1 : 0, prm->levels };
+    for (int l = 0; l < prm->levels; ++l) { key[2 + l] = prm->stride[l]; key[6 + l] = prm->iters[l]; }
+    cudaGraphExec_t exec = nullptr;
+    for (const auto& g : h->track_exec)
+      if (std::memcmp (g.key, key, sizeof (key)) == 0) exec = g.exec;
+    if (!exec)
+    {
+      cudaGraph_t g = nullptr;
+      CK (cudaStreamBeginCapture (s, cudaStreamCaptureModeThreadLocal));
+      track_enqueue (h, s, db != nullptr, prm, cap);
+      const cudaError_t le = cudaGetLastError ();
+      const cudaError_t ce = cudaStreamEndCapture (s, &g);
+      if (le != cudaSuccess || ce != cudaSuccess)
+      {
+        if (g) cudaGraphDestroy (g);
+        return h->fail (B200TSDF_ECUDA, std::string ("tracking graph capture: ") + cudaGetErrorString (le != cudaSuccess ? le : ce));
+      }
+      const cudaError_t ie = cudaGraphInstantiate (&exec, g, 0);
+      cudaGraphDestroy (g);
+      if (ie != cudaSuccess) return h->fail (B200TSDF_ECUDA, std::string ("tracking graph instantiate: ") + cudaGetErrorString (ie));
+      if ((int) h->track_exec.size () >= TRACK_GRAPHS)
+      {
+        cudaGraphExecDestroy (h->track_exec.front ().exec);
+        h->track_exec.erase (h->track_exec.begin ());
+      }
+      b200tsdf::TrackGraph tg;
+      std::memcpy (tg.key, key, sizeof (key)); tg.exec = exec;
+      h->track_exec.push_back (tg);
+    }
+    CK (cudaGraphLaunch (exec, s));
+  }
+  if (dslot >= 0)
+  {
+    CK (cudaEventRecord (h->ev_dconsumed[dslot], s));
+    h->depth_no++;
+  }
+  CK (cudaMemcpyAsync (&B.st, &h->d_track.p->st, sizeof (TrackState), cudaMemcpyDeviceToHost, s));
+  note_device_err (h, s);
+  CK (cudaStreamSynchronize (s));
+  if (int rc = pending_device_err (h)) return rc;
+  const TrackState& st = B.st;
+  static_assert (sizeof (TrackIter) == sizeof (b200tsdf_track_iter), "the log's layout");
+  std::memcpy (res->pose_c2w, st.T, sizeof (st.T));
+  res->status = track_final_status (st, prm->levels);
+  for (int l = 0; l < TRACK_LEVELS; ++l) res->iters[l] = st.iters[l];
+  res->inliers = st.inliers; res->n_log = st.nlog; res->reserved = 0; res->rms = st.rms;
+  std::memcpy (res->A, st.A, sizeof (st.A)); std::memcpy (res->b, st.b, sizeof (st.b));
+  if (log && st.nlog) std::memcpy (log, st.log, (size_t) st.nlog * sizeof (TrackIter));
+  return B200TSDF_OK;
+}
+
+} // namespace
+
+void b200tsdf_default_track_params (b200tsdf_track_params* prm)
+{
+  if (!prm) return;
+  *prm = b200tsdf_track_params{};
+  prm->levels = 3;
+  prm->stride[0] = 4; prm->stride[1] = 2; prm->stride[2] = 1; prm->stride[3] = 1;
+  prm->iters[0] = 10; prm->iters[1] = 6; prm->iters[2] = 4; prm->iters[3] = 0;
+  prm->huber_delta = 0.3f; prm->d_max = 0.95f; prm->w_min = 0.f; prm->min_inliers = 100;
+  prm->damping = 1e-4; prm->eps_rot = 1e-5; prm->eps_trans = 1e-5;
+}
+
+int b200tsdf_track_cloud_device (b200tsdf_t* h, const void* d_points, size_t stride, int xyz_off, int width, int height,
+                                 const double* pose0_c2w, const b200tsdf_track_params* prm, b200tsdf_track_result* res,
+                                 b200tsdf_track_iter* log)
+{
+  if (!h) return B200TSDF_EINVAL;
+  if (int rc = track_args (h, pose0_c2w, prm, res)) return rc;
+  if (!d_points || reinterpret_cast<uintptr_t> (d_points) % 4) return h->fail (B200TSDF_EINVAL, "cloud null or not 4-byte aligned");
+  if (int rc = check_cloud_layout (h, stride, xyz_off, -1, width, height)) return rc;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  return track_run (h, track_input (h, prm, d_points, stride, xyz_off), nullptr, -1, pose0_c2w, prm, res, log);
+}
+
+int b200tsdf_track_depth_device (b200tsdf_t* h, const void* d_depth, int depth_format, float depth_scale, int width, int height,
+                                 const double* pose0_c2w, const b200tsdf_track_params* prm, b200tsdf_track_result* res,
+                                 b200tsdf_track_iter* log)
+{
+  if (!h) return B200TSDF_EINVAL;
+  if (int rc = depth_args (h, depth_format, depth_scale, width, height)) return rc;
+  if (int rc = track_args (h, pose0_c2w, prm, res)) return rc;
+  if (int rc = depth_ptr (h, d_depth, depth_format)) return rc;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  if (int rc = org_buffers (h)) return rc;
+  DepthBatch db = depth_batch (h, depth_format, depth_scale);
+  db.depth[0] = d_depth; db.rgb[0] = nullptr;
+  return track_run (h, track_input (h, prm, org_images (h), 16, 0), &db, -1, pose0_c2w, prm, res, log);
+}
+
+int b200tsdf_track_depth (b200tsdf_t* h, const void* depth, int depth_format, float depth_scale, int width, int height,
+                          const double* pose0_c2w, const b200tsdf_track_params* prm, b200tsdf_track_result* res,
+                          b200tsdf_track_iter* log)
+{
+  if (!h) return B200TSDF_EINVAL;
+  if (int rc = depth_args (h, depth_format, depth_scale, width, height)) return rc;
+  if (int rc = track_args (h, pose0_c2w, prm, res)) return rc;
+  if (int rc = depth_ptr (h, depth, depth_format)) return rc;
+  cudaSetDevice (h->device);
+  if (int rc = pending_device_err (h)) return rc;
+  if (int rc = org_buffers (h)) return rc;
+  int b = 0;
+  unsigned char* d_raw = nullptr;
+  if (int rc = stage_depth (h, depth, org_npix (h) * depth_elem (depth_format), nullptr, 0, b, d_raw)) return rc;
+  DepthBatch db = depth_batch (h, depth_format, depth_scale);
+  db.depth[0] = d_raw; db.rgb[0] = nullptr;
+  return track_run (h, track_input (h, prm, org_images (h), 16, 0), &db, b, pose0_c2w, prm, res, log);
 }
 
 int b200tsdf_sync (b200tsdf_t* h)

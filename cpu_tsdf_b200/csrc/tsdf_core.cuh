@@ -1198,7 +1198,9 @@ B2_HD float interpolate_trilinearly (const Params& p, float x, float y, float z,
 // ---- getNeighbors + getFxn/getGradient/getHessian (tsdf_volume_octree.cpp:655-828) ----------------
 B2_HD int sgn (float x) { return x > 0 ? 1 : -1; }
 
-B2_HD bool query_point (const Params& p, const float* pt, int mode, float* val, float* grad, float* hess)
+// wlo (optional): the smallest weight among the eight neighbour leaves, for callers that must tell observed space from the
+// d = 0 of unobserved leaves (tracking, track.cuh); the reference's getFxn does not look at weights
+B2_HD bool query_point_w (const Params& p, const float* pt, int mode, float* val, float* grad, float* hess, float* wlo)
 {
   int xi, yi, zi;
   if (!voxel_index (p, pt[0], pt[1], pt[2], xi, yi, zi)) return false;
@@ -1208,6 +1210,7 @@ B2_HD bool query_point (const Params& p, const float* pt, int mode, float* val, 
   if (xi < 0 || xi >= p.res - 1 || yi < 0 || yi >= p.res - 1 || zi < 0 || zi >= p.res - 1) return false;
   float c = p.finest_size;                 // xsize_ / xres_
   float fv = 0.f, g0 = 0.f, g1 = 0.f, g2 = 0.f, h01 = 0.f, h02 = 0.f, h12 = 0.f;
+  float wl = 3.402823466e38f;
   for (int dx = 0; dx <= 1; dx++)
     for (int dy = 0; dy <= 1; dy++)
       for (int dz = 0; dz <= 1; dz++)
@@ -1215,6 +1218,7 @@ B2_HD bool query_point (const Params& p, const float* pt, int mode, float* val, 
         float fx_ = voxel_center1 (p, xi + dx), fy_ = voxel_center1 (p, yi + dy), fz_ = voxel_center1 (p, zi + dz);
         Leaf lf = find_leaf (p, fx_, fy_, fz_);
         if (!lf.found) return false;
+        if (wlo) wl = lf.w < wl ? lf.w : wl;
         float vx = mode ? fx_ : lf.n.cx, vy = mode ? fy_ : lf.n.cy, vz = mode ? fz_ : lf.n.cz;
         // unqualified fabs() in the reference is the C double version: the factors and products are
         // DOUBLE, only the `+=` rounds to float (cpp:668, 694-696, 716-718; DESIGN.md "Arithmetic conventions")
@@ -1240,8 +1244,11 @@ B2_HD bool query_point (const Params& p, const float* pt, int mode, float* val, 
     hess[1] = fdiv (h01, c3); hess[2] = fdiv (h02, c3); hess[5] = fdiv (h12, c3);
     hess[3] = hess[1]; hess[6] = hess[2]; hess[7] = hess[5];
   }
+  if (wlo) *wlo = wl;
   return true;
 }
+B2_HD bool query_point (const Params& p, const float* pt, int mode, float* val, float* grad, float* hess)
+{ return query_point_w (p, pt, mode, val, grad, hess, nullptr); }
 
 // ---- renderView, one pixel (tsdf_volume_octree.cpp:278-424) ---------------------------------------
 struct RenderParams

@@ -203,6 +203,77 @@ int  b200tsdf_integrate_depth_batch_device (b200tsdf_t* h, int n, const void* co
 int  b200tsdf_depth_to_cloud_device (b200tsdf_t* h, const void* d_depth, int depth_format, float depth_scale, const uint8_t* d_rgb,
                                      int width, int height, void* d_out);
 
+/* ---- tracking (no counterpart in the reference; DESIGN.md §3i) ----
+ * Refines the camera->world pose of a live frame against the volume by point-to-SDF Gauss-Newton: each sample's residual r and
+ * gradient g are b200tsdf_query mode 1's value and gradient at the transformed point.  For every iteration at level l, with
+ * estimate T:
+ *   samples: pixels (u, v) with u % stride[l] == 0 and v % stride[l] == 0 whose xyz is finite (a depth map is unprojected as
+ *     b200tsdf_integrate_depth unprojects it);
+ *   q = (float) rows 0..2 of T applied to the point as integrate maps a cloud point into the volume;
+ *   inlier: the query at q succeeds, each of its eight neighbour leaves has weight > w_min, and |r| < d_max;
+ *   J = [q x g ; g] (left perturbation T <- Exp (xi) T, xi = (omega, v)), Huber weight rho = 1 if |r| <= huber_delta, else
+ *     huber_delta / |r|; A = sum rho J J^T, b = sum rho J r, summed in double in a fixed order (identical run to run);
+ *   (A + damping diag (A)) xi = -b by LDL^T in double; T <- Exp (xi) T (Rodrigues), rotation re-orthonormalised.
+ * A level ends when |omega| < eps_rot and |v| < eps_trans, or after iters[l] iterations.  The call stops early, T kept at the
+ * last accepted estimate, with fewer than min_inliers inliers (B200TSDF_TRACK_TOO_FEW_INLIERS) or a pivot that is not > 0 or
+ * a non-finite step (B200TSDF_TRACK_SINGULAR).  Each of these is a successful call.
+ * The whole schedule is one CUDA-graph launch (captured once per schedule shape and input kind), ordered after all work
+ * queued on the handle; the call returns once the result is on the host.  The volume is only read: no node, statistic, frame
+ * number or change epoch changes.
+ * Refused with B200TSDF_EINVAL, nothing enqueued: a NULL pose, params or result; a pose that is not finite; levels outside
+ * 1..4, a stride < 1, iters outside 0..64, huber_delta or d_max not > 0, w_min, damping, eps_rot or eps_trans not finite or
+ * (damping, eps_*) < 0, min_inliers < 0; and the input checks of the integrate entry point of the same input.
+ * B200TSDF_ESTATE before reset() and on a sharded handle; a latched device error is reported as by b200tsdf_query. */
+#define B200TSDF_TRACK_CONVERGED        0   /* the last level ended by the convergence test          */
+#define B200TSDF_TRACK_MAX_ITERS        1   /* the last level ran out of iterations                  */
+#define B200TSDF_TRACK_TOO_FEW_INLIERS  2
+#define B200TSDF_TRACK_SINGULAR         3
+typedef struct b200tsdf_track_params
+{
+  int32_t levels;                           /* 1..4, coarse to fine                                                  */
+  int32_t stride[4];                        /* pixel stride of each level, >= 1                                      */
+  int32_t iters[4];                         /* iteration cap of each level, 0..64                                    */
+  float   huber_delta;                      /* metres                                                                */
+  float   d_max;                            /* inlier bound on |r|, metres                                           */
+  float   w_min;                            /* inlier bound on the neighbour weights (w > w_min)                     */
+  int32_t min_inliers;
+  double  damping;                          /* lambda                                                                */
+  double  eps_rot, eps_trans;               /* radians, metres                                                       */
+} b200tsdf_track_params;
+void b200tsdf_default_track_params (b200tsdf_track_params* prm);
+typedef struct b200tsdf_track_result
+{
+  double  pose_c2w[16];                     /* refined pose, row-major                                               */
+  int32_t status;                           /* B200TSDF_TRACK_*                                                      */
+  int32_t iters[4];                         /* iterations run per level                                              */
+  int32_t inliers;                          /* of the last iteration                                                 */
+  int32_t n_log;                            /* entries written to the log (the sum of iters)                         */
+  int32_t reserved;
+  double  rms;                              /* sqrt (sum r^2 / inliers) of the last iteration, 0 without inliers     */
+  double  A[36];                            /* sum rho J J^T of the last iteration (undamped), row-major             */
+  double  b[6];                             /* sum rho J r of the last iteration                                     */
+} b200tsdf_track_result;
+/* one iteration of the optional log: its level, inliers, sum rho r^2 and the step xi (zero when the call stopped there) */
+typedef struct b200tsdf_track_iter
+{
+  int32_t level, inliers;
+  double  cost;
+  double  step[6];
+} b200tsdf_track_iter;
+/* log: NULL, or room for sum (iters[0 .. levels-1]) entries.  Host depth map (format and size as b200tsdf_integrate_depth;
+ * staged through the same pinned slots; the buffer is free when the call returns). */
+int  b200tsdf_track_depth (b200tsdf_t* h, const void* depth, int depth_format, float depth_scale, int width, int height,
+                           const double* pose0_c2w, const b200tsdf_track_params* prm, b200tsdf_track_result* res,
+                           b200tsdf_track_iter* log);
+/* the same with the depth map in device memory of h's device */
+int  b200tsdf_track_depth_device (b200tsdf_t* h, const void* d_depth, int depth_format, float depth_scale, int width, int height,
+                                  const double* pose0_c2w, const b200tsdf_track_params* prm, b200tsdf_track_result* res,
+                                  b200tsdf_track_iter* log);
+/* an organised cloud in device memory, in the layout of b200tsdf_integrate_device (the colour is not read) */
+int  b200tsdf_track_cloud_device (b200tsdf_t* h, const void* d_points, size_t stride, int xyz_off, int width, int height,
+                                  const double* pose0_c2w, const b200tsdf_track_params* prm, b200tsdf_track_result* res,
+                                  b200tsdf_track_iter* log);
+
 /* getFxn / getGradient / getHessian (cpp:655-725) with mode 0, or the combined
  * getFxnAndGradient / getFxnGradientAndHessian (cpp:728-794) with mode 1.  what: bit0 value,
  * bit1 gradient (3 floats), bit2 hessian (9 floats, row-major).  ok[i] = the reference's bool; where it is 0 the outputs of

@@ -86,6 +86,14 @@ inline void pose_rows (const Affine3d& t, double* m)
   std::memcpy (m, t.m, sizeof (double) * 16);
 #endif
 }
+inline void set_pose_rows (Affine3d& t, const double* m)
+{
+#ifdef B200TSDF_WITH_PCL
+  for (int r = 0; r < 4; ++r) for (int c = 0; c < 4; ++c) t.matrix () (r, c) = m[r * 4 + c];
+#else
+  std::memcpy (t.m, m, sizeof (double) * 16);
+#endif
+}
 inline Vector3i vector3i (const std::int32_t* v)
 {
 #ifdef B200TSDF_WITH_PCL
@@ -249,6 +257,22 @@ public:
                                                      d_rgb.empty () ? nullptr : d_rgb.data (), width, height, m.data ());
     return status_ == 0;
   }
+
+  // (no counterpart in the reference) Tracking (b200tsdf_track_depth, DESIGN.md §3i): refines `trans`, the camera->world pose
+  // of a depth map of the configured image size, against the volume by point-to-SDF Gauss-Newton; the volume is only read.
+  // On success `trans` holds the refined pose and `result` (optional) the status (B200TSDF_TRACK_*), iterations, inliers and
+  // normal equations; prm: nullptr for b200tsdf_default_track_params.  A call that stops early (too few inliers, a singular
+  // system) succeeds and leaves `trans` at the last accepted estimate.
+  bool trackDepthImage (const std::uint16_t* depth, float scale, int width, int height, Affine3d& trans,
+                        const b200tsdf_track_params* prm = nullptr, b200tsdf_track_result* result = nullptr)
+  { return track (depth, B200TSDF_DEPTH_U16, scale, width, height, trans, prm, result, false); }
+  bool trackDepthImage (const float* depth, int width, int height, Affine3d& trans,
+                        const b200tsdf_track_params* prm = nullptr, b200tsdf_track_result* result = nullptr)
+  { return track (depth, B200TSDF_DEPTH_F32, 1.f, width, height, trans, prm, result, false); }
+  // the same with the depth map (format B200TSDF_DEPTH_U16 or _F32) in device memory
+  bool trackDepthImageDevice (const void* d_depth, int format, float scale, int width, int height, Affine3d& trans,
+                              const b200tsdf_track_params* prm = nullptr, b200tsdf_track_result* result = nullptr)
+  { return track (d_depth, format, scale, width, height, trans, prm, result, true); }
 
   bool getFxn (const PointXYZ& pt, float& val) const                                               // cpp:655-672
   { std::uint8_t ok = 0; float p[3] = { pt.x, pt.y, pt.z }; b200tsdf_query (h_, p, 1, 1, 0, &val, nullptr, nullptr, &ok); return ok != 0; }
@@ -475,6 +499,22 @@ public:
 
 private:
   void push () { if (h_) status_ = b200tsdf_set_config (h_, &cfg_); }
+  bool track (const void* depth, int format, float scale, int width, int height, Affine3d& trans, const b200tsdf_track_params* prm,
+              b200tsdf_track_result* result, bool on_device)
+  {
+    if (!h_) return false;
+    b200tsdf_track_params def;
+    if (!prm) { b200tsdf_default_track_params (&def); prm = &def; }
+    b200tsdf_track_result r;
+    double m[16];
+    detail::pose_rows (trans, m);
+    status_ = on_device ? b200tsdf_track_depth_device (h_, depth, format, scale, width, height, m, prm, &r, nullptr)
+                        : b200tsdf_track_depth (h_, depth, format, scale, width, height, m, prm, &r, nullptr);
+    if (status_ != 0) return false;
+    detail::set_pose_rows (trans, r.pose_c2w);
+    if (result) *result = r;
+    return true;
+  }
   bool depth_image (const void* depth, int format, float scale, int width, int height, const Affine3d& trans, const std::uint8_t* rgb)
   {
     if (!h_) return false;
